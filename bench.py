@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — broadcast fan-out throughput of the B200-native engine (BASELINE.json metric).
+"""bench.py — broadcast fan-out throughput of the fan-out engine (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm
     python bench.py --impl reference --gpus N --steps K ...  # CPU restatement of the reference path
@@ -60,11 +60,11 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -175,6 +175,42 @@ def reference_arm(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+DUMP_CONNS = 1024
+DUMP_BYTES = 48 << 20
+
+
+def write_outputs(eng, out_dir, res, rec, F, pool):
+    """What one polled batch delivered, as its caller receives it: the batch counters, and for a fixed
+    seeded sample of connections (at most DUMP_CONNS, at most DUMP_BYTES of records) their spans
+    (conn, ring offset, length, records) and the framed bytes of every record (4-byte length prefix +
+    frame; the pad up to the 32-byte record stride is unspecified and left out).  float64 / float32."""
+    import numpy as np
+
+    if res.runs:   # run-length table {conn0, n_conns, ring_off, len, n_records, off_stride}: one row per connection
+        r = np.ctypeslib.as_array(C.cast(res.runs, C.POINTER(C.c_uint32)), shape=(res.n_runs, 6)).astype(np.int64)
+        cnt = r[:, 1]
+        k = np.arange(int(cnt.sum())) - np.repeat(np.cumsum(cnt) - cnt, cnt)
+        rr = np.repeat(r, cnt, axis=0)
+        spans = np.stack([rr[:, 0] + k, rr[:, 2] + k * rr[:, 5], rr[:, 3], rr[:, 4]], axis=1)
+    else:
+        spans = np.ctypeslib.as_array(C.cast(res.spans, C.POINTER(C.c_uint32)), shape=(res.n_spans, 4)).astype(np.int64)
+    spans = spans[np.lexsort((spans[:, 1], spans[:, 0]))]
+    per_span = 4 * int(spans[:, 3].max()) * F if len(spans) else 1
+    n = min(len(spans), DUMP_CONNS, max(1, DUMP_BYTES // per_span))
+    pick = np.sort(np.random.default_rng(0).choice(len(spans), size=n, replace=False))
+    recs = []
+    for conn, off, ln, nrec in spans[pick]:
+        # output pool: offsets are 32-byte units relative to the batch's pool_base
+        data = eng.read(int(conn), int(off) + (int(res.pool_base) if pool else 0), int(ln))
+        recs.append(np.frombuffer(data, dtype=np.uint8).reshape(int(nrec), rec)[:, :F])
+    counters = np.array([res.n_msgs, res.n_deliveries, res.bytes_out, res.n_spans, res.n_runs, res.n_overflow,
+                         res.n_direct_dropped, res.status], dtype=np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "counters.npy"), counters)
+    np.save(os.path.join(out_dir, "spans.npy"), spans[pick].astype(np.float64))
+    np.save(os.path.join(out_dir, "records.npy"), np.concatenate(recs).astype(np.float32) if recs else np.zeros((0, F), np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -199,6 +235,9 @@ def main():
                          "copies the batch from its process's pinned staging (host-buffer path only)")
     ap.add_argument("--host-rings", action="store_true",
                     help="egress hand-off mode: rings in mapped pinned host memory (PCDN_FLAG_HOST_RINGS); PCIe-bound, use with --conns <= 65536")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step delivered (counters, the spans and framed "
+                         "records of a fixed sample of connections) to DIR/<name>.npy, for comparing two builds")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -325,12 +364,25 @@ def main():
         launches0 = eng.stats().kernel_launches
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(stream)
-        for _ in range(args.steps):
-            step_device()
+        last = None
+        for i in range(args.steps):
+            if args.dump_outputs and i == args.steps - 1:
+                # the last step is polled the way a caller receives a batch; its ring space goes back
+                # after its outputs are written, before anything else is submitted
+                k = state["i"] & 1
+                state["i"] += 1
+                last = eng.submit_device(dbs[k])
+                last_res = eng.poll(last)
+            else:
+                step_device()
         drain_device()                        # waits (on the stream) for the last pack
         ev1.record(stream)
         sync_all()
         gpu_launches = int(eng.stats().kernel_launches - launches0)   # counted by the library at every launch site
+        if last is not None:
+            if rank == 0:
+                write_outputs(eng, args.dump_outputs, last_res, rec, F, args.pool)
+            eng.release_batch(last)
     ms = ev0.elapsed_time(ev1)
     t_ms = torch.tensor([ms], dtype=torch.float64, device=dev)
     if world > 1:
@@ -438,14 +490,7 @@ def main():
     pack_bytes = M * (n_conns * F + L)          # algorithmic bytes of one pack launch: D*F stores + L read per message
     peak, peak_src = measured_peak()
     achieved = pack_bytes / (ms_pack * 1e-3) / 1e9
-    traffic, traffic_source = None, None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = json.load(open(tp)).get("k_pack_dram_bytes_per_launch")
-            traffic_source = "static ncu capture (profiles/traffic.json: dram__bytes_read.sum + dram__bytes_write.sum of one --set full launch)"
-        except Exception:
-            traffic = None
+    traffic, traffic_source = None, "not measured"
 
     # ---- e2e: host buffers through the C ABI, H2D + D2H inside the timed region ---------------------
     # (N>1: same call on every rank — the SPMD contract; only rank 0's bytes are used, the other ranks

@@ -1,5 +1,5 @@
 /*
- * pcdn_fanout.h — C ABI of the B200-native broker fan-out engine.
+ * pcdn_fanout.h — C ABI of the broker fan-out engine (CUDA, H100 / sm_90a).
  *
  * This is the drop-in boundary for ONE hot path of EspressoSystems/Push-CDN: cdn-broker's
  * broadcast + direct-message routing and per-recipient replication with the cdn-proto

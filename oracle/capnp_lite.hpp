@@ -5,7 +5,7 @@
 // capnp_lite.hpp — encoder/decoder for the cdn-proto wire messages the broker routes.
 //
 // PARITY UNPINNED: the reference serialises with the third-party crate `capnp` 0.20.6
-// (Cargo.lock:799-800, NOT vendored under /root/reference; call sites cdn-proto/src/message.rs:
+// (Cargo.lock:799-800, NOT vendored in the reference repository; call sites cdn-proto/src/message.rs:
 // 118-119,203,214-228) and its only test at this boundary is a round trip without golden bytes
 // (message.rs:397-457).  The layout below is restated from the public Cap'n Proto encoding spec and
 // the struct sizes/discriminants in the reference's generated code:

@@ -2,7 +2,7 @@
 //
 // PCDN_LIB_DIR: directory that holds libpcdn_fanout.so (default: ../push-cdn_b200 relative to this
 // crate, where `python -c 'import __graft_entry__ as g; g.build()'` leaves it).  The library is built
-// by nvcc for sm_100a; this script does not compile anything.
+// by nvcc for sm_90a; this script does not compile anything.
 use std::{env, path::PathBuf};
 
 fn main() {

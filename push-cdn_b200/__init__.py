@@ -1,7 +1,7 @@
-"""push-cdn_b200 — B200-native fan-out engine for Push-CDN's cdn-broker hot path.
+"""push-cdn_b200 — H100 (sm_90a) fan-out engine for Push-CDN's cdn-broker hot path.
 
 This Python module is a thin ctypes binding over the C ABI (``include/pcdn_fanout.h``) of
-``libpcdn_fanout.so`` (CUDA, sm_100a).  It mirrors the names of the reference's broker API
+``libpcdn_fanout.so`` (CUDA, sm_90a).  It mirrors the names of the reference's broker API
 (`Connections::*`, `Inner::handle_broadcast_message`, `Inner::handle_direct_message`,
 `user_receive_loop` / `broker_receive_loop` — cdn-broker/src/{connections/mod.rs,
 tasks/broker/handler.rs, tasks/user/handler.rs}) so that tests read like the reference's own.
@@ -27,7 +27,7 @@ INCLUDE = os.path.join(_ROOT, "include")
 SOURCES = ["engine.cu", "kernels.cu", "egress.cu", "host_state.cpp", "frame_parse.cpp", "nccl_dl.cpp"]
 HEADERS = ["kernels.cuh", "host_state.h", "frame_parse.h", "frame_parse_core.h", "hash.h", "nccl_dl.h", "engine_internal.h"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-pthread", "-shared",
 ]
 
@@ -65,7 +65,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into the in-tree shared library (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into the in-tree shared library (nvcc cross-compiles
     without a GPU)."""
     if not force and not needs_build():
         return LIB_PATH

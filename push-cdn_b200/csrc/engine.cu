@@ -120,9 +120,8 @@ int acquire_open_slot(pcdn_engine* e) {
 }
 
 // The adaptive pack-stream overlap applies to batches whose previous output was at most this many bytes.
-// With every step queued ahead, about half of the overlapped packs lose the launch race against the next
-// control stage and run ~40 % longer (profiles/r2_timeline_overlap.txt); the overlap hides at most the
-// ~0.08 ms control stage, so it stops paying once a pack takes more than ~0.25 ms (1.5 GB of stores).
+// With every step queued ahead, overlapped packs can lose the launch race against the next control stage
+// and run much longer; the overlap hides at most the short control stage, so it stops paying for long packs.
 static constexpr unsigned long long kOverlapMaxBytes = 3ull << 29;
 static constexpr uint32_t kTimelineBatches = 64;
 
@@ -132,16 +131,16 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   DeviceGuard dg(sh.device);
   ShardSlot& s = sh.slots[si];
   // Default: the pack runs on the main stream.  A/B switch (pack_variant bit 3): run it on the
-  // high-priority pack stream so the next batch's control kernels overlap it — measured SLOWER for
-  // the bulk-store pack (profiles/r1_sweep_overlap.txt), so it stays opt-in.
+  // high-priority pack stream so the next batch's control kernels overlap it — slower for a long
+  // bulk-store pack, so it stays opt-in.
   const bool dp = sh.direct_publish;
   // Batches of nothing but many direct messages DO take the pack stream: their control kernels are
   // latency-bound (three dependent random reads per message), their pack is a separate bandwidth-bound
-  // launch, and the two overlap well — C4: 1.98 → 2.10 G msgs/s (profiles/r2_cfg_C4_sweep_v*.json).
+  // launch, and the two overlap well (config C4).
   const bool direct_only = s.in.n_bcast == 0 && n_direct >= kThinSeparateMin;
   // Broadcast batches: running the next batch's control stage beside this batch's pack helps when the pack is
-  // short and message-major (sparse fan-out, config 5: 0.293 -> 0.282 ms) and hurts a long pack, which then shares
-  // SMs and HBM with it (config 5 dense: 5.29 -> 6.70 ms; C2 likewise) - profiles/r2_overlap_adaptive.txt.  Which
+  // short and message-major (sparse fan-out, config 5) and hurts a long pack, which then shares SMs and HBM with
+  // it (config 5 dense, C2).  Which
   // one this batch will be is decided on the device, so the class mix and size of the most recent COMPLETED batch
   // of this shard predict it (a workload changes its mix rarely; a wrong guess costs one batch a few percent).
   if (!dp && s.in.n_bcast > 0) {
@@ -185,7 +184,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   const bool fused = dp && sh.dev.N <= kSmallCtrlConns && s.in.n_msgs <= kSmallCtrlMsgs &&
                      (uint64_t)s.in.n_bcast * sh.dev.nblk <= kSmallCtrlItems;
   // Spans go straight into mapped host memory when few are expected (16-byte PCIe writes: a table
-  // of 16 K spans measured 20 us slower than the staged copy): the smallest geometry, or a batch
+  // of 16 K spans is slower than the staged copy): the smallest geometry, or a batch
   // without broadcasts and with few messages (at most one span per message).  Otherwise they are staged in HBM and copied
   // out with one DMA of the exact size while the pack runs.
   s.spans_mapped = dp && (sh.dev.N <= 8192 || (s.in.n_bcast == 0 && s.in.n_msgs <= 4096));
@@ -205,7 +204,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
     launch_match(sh.dev, s.w, s.in, st);
     if (timed) CUDA_TRY(cudaEventRecord(tev[2], st));
     launch_plan(sh.dev, s.w, s.in, st);
-    launch_offsets(sh.dev, s.w, s.in, has_direct, st);
+    launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);
     if (timed) CUDA_TRY(cudaEventRecord(tev[3], st));
   }
   if (!s.spans_mapped) {
@@ -222,7 +221,12 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   s.on_pack_stream = ps != st;
   if (e->timeline_async) sh.tl_ps[(sh.tl_n - 1) % kTimelineBatches] = (int)s.on_pack_stream;
   if (timed) CUDA_TRY(cudaEventRecord(tev[4], ps));
-  launch_pack(sh.dev, s.w, s.in, n_direct, e->cfg.pack_variant, sh.n_sms, ps);
+  // k_pack CTAs per SM unless pack_variant bits 8-11 set them: 4 when the pack has the GPU to itself, 3 when it
+  // overlaps the next batch's control kernels (one H100: C2 +1.4 % with 4; the overlapped config-5 sparse shard
+  // +2 % with 3)
+  uint32_t pack_variant = e->cfg.pack_variant;
+  if (!((pack_variant >> 8) & 15u)) pack_variant |= (fat_overlap ? 3u : 4u) << 8;
+  launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, ps);
   if (timed) CUDA_TRY(cudaEventRecord(tev[5], ps));
   CUDA_TRY(cudaGetLastError());
   if (!fused) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));

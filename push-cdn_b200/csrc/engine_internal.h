@@ -107,7 +107,7 @@ struct ShardSlot {
 struct Shard {
   int device = 0;
   uint32_t gindex = 0;           // global shard number inside the broker
-  int n_sms = 148;
+  int n_sms = 132;
   bool direct_publish = false;   // spans / overflow list written by the device into mapped host memory
   uint8_t* h_rings = nullptr;    // PCDN_FLAG_HOST_RINGS: host address of the (mapped, pinned) rings
   // main stream: uploads, table updates, direct/match/plan/offsets, release.  pack stream: k_pack, so

@@ -1,4 +1,4 @@
-// kernels.cu — hand-written sm_100a kernels of the fan-out engine.  See kernels.cuh for the
+// kernels.cu — hand-written sm_90a kernels of the fan-out engine.  See kernels.cuh for the
 // pipeline and DESIGN.md for the roofline of each kernel.  Everything here is integer/byte work
 // bound by HBM bandwidth; there is deliberately no tensor-core code.
 #include "kernels.cuh"
@@ -657,7 +657,7 @@ __device__ __forceinline__ void pool_allocate(const DevState& s, const Work& w, 
 // Pool mode, two ways to chain the CTAs' unit totals: LOOKBACK (the fused small-engine kernel: its CTAs
 // are co-resident, the chain is at most 64 long) or, in the regular kernel, CTA-local offsets + the
 // CTA total in lb_tot[], finished by k_pool_finish (one more launch instead of 4096 CTAs polling each
-// other: the look-back cost 40 us at 2^20 connections, the finish kernel 5).
+// other is slower at 2^20 connections).
 template <bool HAS_DIRECT, int NT, bool SPARSE_BOUNDS, bool LOOKBACK>
 __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b, const Work& w, uint32_t max_conns,
                                              uint32_t c, uint32_t vb, uint32_t nvb) {
@@ -868,13 +868,13 @@ __global__ void __launch_bounds__(1024) k_pool_finish(DevState s, Work w, uint32
   }
 }
 
-void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, cudaStream_t st) {
+void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st) {
   if (has_direct) PCDN_COUNT_LAUNCH, k_offsets<true><<<s.N / 256, 256, 0, st>>>(s, b, w, s.N);
   else PCDN_COUNT_LAUNCH, k_offsets<false><<<s.N / 256, 256, 0, st>>>(s, b, w, s.N);
   if (s.pool) {
     const uint32_t nblk = s.N / 256;
     if (nblk * 4 > 48u * 1024) cudaFuncSetAttribute(k_pool_finish, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(nblk * 4));  // > 3 M connections per shard
-    PCDN_COUNT_LAUNCH, k_pool_finish<<<std::min<uint32_t>(148u, (s.N + 8191) / 8192), 1024, nblk * 4, st>>>(s, w, nblk);
+    PCDN_COUNT_LAUNCH, k_pool_finish<<<std::min<uint32_t>((uint32_t)n_sms, (s.N + 8191) / 8192), 1024, nblk * 4, st>>>(s, w, nblk);
   }
 }
 
@@ -1134,7 +1134,7 @@ __device__ __forceinline__ void pack_fat_phase(const DevState& s, const BatchIn&
 // word prefix + lane rank, the same formula k_offsets used); records that are adjacent in the ring
 // are written as ONE contiguous run — for the all-subscribed case that is the whole batch
 // (8 x 1088 B = 8.7 KB) per connection instead of eight separate 1 KB writes, which is what the
-// HBM row buffers want (profiles/: 1 KB granules reach 83 % of the copy peak, >=4 KB runs 96 %).
+// HBM row buffers want (scattered 1 KB granules are written well below the copy rate, runs of several KB close to it).
 //   VARIANT 0: the warp copies a connection's run with 16-byte shared loads + st.global.cs.v4
 //   VARIANT 1: every lane issues one TMA bulk store (shared → global) per run of ITS connection
 template <int VARIANT>
@@ -1311,7 +1311,7 @@ __device__ __forceinline__ void pack_thin_phase(const DevState& s, const BatchIn
 // all indexed by the message, so the warps of a CTA stream the arena in order; only the record
 // stores are scattered (one ~700 B record per ring).
 // (a variant with four entries in flight per warp measured no faster: the phase is bound by the
-// scattered sub-KB writes, not by load latency — profiles/r1_cfg_C4*.json)
+// scattered sub-KB writes, not by load latency)
 __device__ __forceinline__ void pack_direct_phase(const DevState& s, const BatchIn& b, const Work& w) {
   const uint32_t n = b.n_msgs;
   const uint32_t pool_base = w.stats->pool_base;
@@ -1356,7 +1356,7 @@ __global__ void __launch_bounds__(256) k_pack(DevState s, BatchIn b, Work w, int
 // Batches dominated by direct messages run the direct phase as its own launch at full occupancy
 // (no shared memory, 8 CTAs per SM): a warp per record is a chain of two dependent DRAM reads
 // (list entry, frame) before its stores, so the phase scales with warps in flight — 24 → 48
-// warps per SM measured +25 % on the 1 M x 512 B direct workload (profiles/r1_sweep_secondary.txt).
+// warps per SM is faster on the 1 M x 512 B direct workload (config C4).
 __global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, Work w) {
   if (w.stats->status) return;
   pack_direct_phase(s, b, w);
@@ -1364,7 +1364,7 @@ __global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, W
 
 void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t variant, int n_sms, cudaStream_t st) {
   const bool direct_separate = n_direct >= kThinSeparateMin;
-  // Default (variant 0): TMA bulk stores, 3 CTAs per SM — the best of the sweep in profiles/.
+  // Default (variant 0): TMA bulk stores; CTAs per SM come from the engine (launch_shard_pipeline), else 3.
   // A/B switches for profiling: bit 2 = st.global.cs.v4 stores instead of bulk stores; bit 1 = no
   // connection-major class (DevState::cm_enable, read by k_plan_a); bits 4-7 = log2 multiplier of
   // the 128 KB message-major tile (DevState::fat_tile_bytes); bits 8+ = CTAs per SM.

@@ -1,4 +1,4 @@
-// kernels.cuh — device-side data layout and kernel launchers of the fan-out engine (sm_100a).
+// kernels.cuh — device-side data layout and kernel launchers of the fan-out engine (sm_90a).
 //
 // Per batch the engine runs (all on one stream, no host round trip in between):
 //   K0  k_parse         (device-parse mode) thread per frame: Cap'n Proto walk, Topic::prune, recipient
@@ -209,7 +209,7 @@ void launch_parse(const DevState& s, const Work& w, const BatchIn& b, cudaStream
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st);
 void launch_match(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
-void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, cudaStream_t st);
+void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st);
 // fused match + plan + offsets for N <= kSmallCtrlConns and n_msgs <= kSmallCtrlMsgs (one cluster launch)
 void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool zero_stats,
                        BatchStats* publish, cudaStream_t st);

@@ -163,7 +163,7 @@ def generate():
         raise SystemExit("gen_pcdn_sys: cannot parse declaration: %r" % d)
 
     o = []
-    o.append("//! pcdn-sys — raw FFI binding of `include/pcdn_fanout.h`, the C ABI of the B200 fan-out engine")
+    o.append("//! pcdn-sys — raw FFI binding of `include/pcdn_fanout.h`, the C ABI of the H100 fan-out engine")
     o.append("//! (libpcdn_fanout.so).  GENERATED by scripts/gen_pcdn_sys.py from the header: do not edit;")
     o.append("//! tests/test_pcdn_sys.py fails when this file and the header diverge.  The meaning of every item,")
     o.append("//! and the reference function each entry point replaces, is documented in the header.")

@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and makes the repo importable.
 
 `-m "not gpu"` runs here on CPU (oracle vs the reference's own scenarios, host logic, ABI symbols);
-`-m gpu` runs on a B200 and compares the CUDA path (through the C ABI) with the oracle.
+`-m gpu` runs on an H100 and compares the CUDA path (through the C ABI) with the oracle.
 """
 import os
 import sys
@@ -17,7 +17,7 @@ if TESTS not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")

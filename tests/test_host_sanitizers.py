@@ -55,7 +55,7 @@ def test_state_calls_under_tsan(tmp_path):
     8 threads x 20 000 calls against a host-only engine; any data race report fails the test."""
     exe = tmp_path / "tsan_state_calls"
     srcs = [os.path.join(CSRC, f) for f in ("engine.cu", "kernels.cu", "egress.cu", "host_state.cpp", "frame_parse.cpp", "nccl_dl.cpp")]
-    cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-g", "-std=c++17",
+    cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-g", "-std=c++17",
            "-Xcompiler", "-fPIC,-pthread,-fsanitize=thread", "-I", os.path.join(ROOT, "include"), *srcs,
            os.path.join(ROOT, "tests", "cpp", "tsan_state_calls.c"), "-o", str(exe), "-lpthread", "-ltsan", "-ldl"]
     r = subprocess.run(cmd, capture_output=True, text=True)
