@@ -176,17 +176,18 @@ def test_output_pool_backpressure_and_wrap(pcdn, staged):
     w.e.close()
 
 
-@pytest.mark.parametrize("pool", [False, True])
-def test_alternating_batch_classes_in_flight(pcdn, pool):
+@pytest.mark.parametrize("pool,pack_variant", [(False, 0), (True, 0), (True, 6 << 8)], ids=["False", "True", "True-6ctas"])
+def test_alternating_batch_classes_in_flight(pcdn, pool, pack_variant):
     """The engine moves the pack of short message-major-only batches to its pack stream (so the next
     batch's control kernels run beside it) and decides that from the last COMPLETED batch
     (engine.cu launch_shard_pipeline).  Several batches are in flight here and their classes alternate
     — sparse 4 KiB broadcasts (message-major only), dense 1 KiB broadcasts (connection-major), direct
     only — so successive packs land on different streams in every order; per-connection order and bytes
-    must still be the oracle's."""
+    must still be the oracle's.  pack_variant 6 << 8: k_pack with 6 CTAs per SM instead of the 3 or 4
+    the engine picks."""
     rng = random.Random(77)
     cfg = dict(max_conns=8192, ring_bytes_per_conn=1 << 18, max_batch_deliveries=1 << 18, batch_slots=4,
-               max_batch_bytes=8 << 20)
+               max_batch_bytes=8 << 20, pack_variant=pack_variant)
     if pool:
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=1 << 30)
     w = World(pcdn, **cfg)

@@ -37,33 +37,43 @@ def test_reference_scenario_host_rings(pcdn, scenario):
 
 # ------------------------------------------------------------------ differential harness
 class World:
-    """drives engine and oracle with identical calls and compares delivered frames"""
+    """drives engine and oracle with identical calls and compares delivered frames
+    (record=True: also keeps the engine calls and the oracle's frames of every check(), so that
+    replay() can run the same workload on engines of other configurations against this ONE oracle run)"""
 
-    def __init__(self, pcdn, n_valid_topics=0, **cfg):
+    def __init__(self, pcdn, n_valid_topics=0, record=False, **cfg):
         kw = dict(max_conns=8192, max_topics=256, max_keys=16384, ring_bytes_per_conn=1 << 18,
                   max_batch_msgs=4096, max_batch_bcast=512, max_batch_bytes=32 << 20,
                   max_batch_deliveries=1 << 20, identity="/", n_valid_topics=n_valid_topics)
         kw.update(cfg)
         self.pcdn = pcdn
+        self.cfg = kw
         self.e = pcdn.Engine(**kw)
         self.o = orc.Oracle("/", n_valid_topics)
         self.map = {}
         self.taken = {}
+        self.calls = [] if record else None
+
+    def _engine(self, name, *a):
+        r = getattr(self.e, name)(*a)
+        if self.calls is not None:
+            self.calls.append((name, a, r))
+        return r
 
     def add_user(self, key, topics):
-        c = self.e.add_user(key, topics)
+        c = self._engine("add_user", key, topics)
         self.map[c] = self.o.add_user(key, topics)
         return c
 
     def add_broker(self, ident, topics=()):
-        c = self.e.add_broker(ident)
+        c = self._engine("add_broker", ident)
         self.map[c] = self.o.add_broker(ident)
         if topics:
             self.both("subscribe_broker_to", ident, list(topics))
         return c
 
     def both(self, name, *a):
-        getattr(self.e, name)(*a)
+        self._engine(name, *a)
         getattr(self.o, name)(*a)
 
     def bcast(self, topics, raw, to_users_only=False):
@@ -86,9 +96,27 @@ class World:
     def check(self):
         got = self.e.drain()
         want = self.expect()
+        if self.calls is not None:
+            self.calls.append(("check", (), want))
+        return self.compare(self.e, got, want)
+
+    def replay(self, **cfg):
+        """the recorded engine calls on a fresh engine configured like this one updated by `cfg`; every
+        batch must deliver the oracle frames recorded for it"""
+        e = self.pcdn.Engine(**{**self.cfg, **cfg})
+        try:
+            for name, a, r in self.calls:
+                if name == "check":
+                    self.compare(e, e.drain(), r)
+                else:
+                    assert getattr(e, name)(*a) == r, name
+        finally:
+            e.close()
+
+    def compare(self, e, got, want):
         bad = [c for c in sorted(set(got) | set(want)) if got.get(c, []) != want.get(c, [])]
         if bad:
-            self.dump(bad, got, want)
+            self.dump(e, bad, got, want)
         assert set(got) == set(want), (sorted(set(got) ^ set(want))[:10])
         for c in want:
             assert len(got[c]) == len(want[c]), (c, len(got[c]), len(want[c]))
@@ -96,12 +124,12 @@ class World:
                 assert g == w, f"conn {c} frame {i}: {len(g)} vs {len(w)} bytes"
         return sum(len(v) for v in want.values())
 
-    def dump(self, bad, got, want):
+    def dump(self, e, bad, got, want):
         """diagnostics for a failing comparison (pytest shows them with the failure)"""
         import sys
         f = sys.stdout
         f.write(f"==== {len(bad)} bad connections of {len(want)}; first: {bad[:20]}\n")
-        r = self.e.last_result
+        r = e.last_result
         f.write(f"last batch: msgs={r.n_msgs} deliveries={r.n_deliveries} spans={r.n_spans} overflow={r.n_overflow} "
                 f"dropped={r.n_direct_dropped} status={r.status}\n")
         for c in bad[:6]:
@@ -510,16 +538,24 @@ def test_connection_id_quarantined_until_batches_released(pcdn):
     e.close()
 
 
-@pytest.mark.parametrize("staged,max_conns", [(False, 8192), (True, 8192), (False, 20000), (False, 65536), (False, 65537)])
+POOL_FLAGS = {"pool": 16, "pool-runs": 16 | 8}   # FLAG_OUTPUT_POOL, | FLAG_SPAN_RUNS
+
+
+@pytest.mark.parametrize("staged,max_conns", [(False, 8192), (True, 8192), (False, 20000), (False, 65536), (False, 65537)] +
+                         [(p, n) for n in (20000, 65536, 65537) for p in POOL_FLAGS])
 def test_small_engine_batch_sizes_across_the_fused_limit(pcdn, staged, max_conns):
     """engines with <= 65536 connection slots route batches of <= 256 messages through the fused
     control kernel (k_ctrl_small: 1, 3 and 8 passes of 8192 connections here) and larger ones through
     the regular pipeline; all must agree with the oracle at and around the limit (1, 2, 255, 256, 257,
     700 messages; broadcasts, directs incl. a hot recipient and unknown keys).  65537 slots is the
-    first geometry that always takes the regular pipeline with the staged span table."""
+    first geometry that always takes the regular pipeline with the staged span table.
+    staged = "pool" / "pool-runs": output-pool engines (plain / run-length span table), whose regular
+    pipeline finishes the pool offsets in k_pool_finish with one CTA per 8192 slots: 3, 8 and 9 CTAs here."""
     rng = random.Random(11)
+    kw = dict(flags=POOL_FLAGS[staged], pool_bytes=1 << 28) if isinstance(staged, str) else \
+        dict(flags=pcdn.FLAG_STAGED_SPANS if staged else 0)
     w = World(pcdn, ring_bytes_per_conn=1 << 18, max_batch_msgs=1024, max_batch_bcast=1024, max_conns=max_conns,
-              max_keys=max(16384, max_conns + 2048), flags=pcdn.FLAG_STAGED_SPANS if staged else 0)
+              max_keys=max(16384, max_conns + 2048), **kw)
     # connection ids are handed out densely: with the bulk loader the later 8192-connection blocks of a
     # large engine get users too (topic 9 only, so they stay out of the checked traffic)
     if max_conns > 8192:
