@@ -428,7 +428,9 @@ int pcdn_poll(pcdn_engine* e, uint64_t batch_id, pcdn_batch_result* out, int blo
 int pcdn_read(pcdn_engine* e, pcdn_conn conn, uint32_t ring_off, uint32_t len, void* dst);
 /* PCDN_FLAG_OUTPUT_POOL: run a refused batch (status PCDN_EAGAIN) again after older batches have been
  * released.  Only the oldest unreleased batch can be retried; its result is polled again afterwards.
- * The batch is routed against the tables as they are at the retry. */
+ * The batch is routed against the tables as they were when it was launched, on every shard, like any
+ * other batch: a state change made between the refusal and the retry applies to later batches only.
+ * Shards that accepted their share keep it; the others place and pack theirs again. */
 int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id);
 /* The host has written every span of the batch: free its ring space and its slot.  This is the
  * analogue of dropping the last `Bytes` clone (limiter/pool.rs:44-52).  In order, oldest first. */

@@ -385,12 +385,20 @@ int drain_locked(pcdn_egress* g, uint64_t batch_id, pcdn_egress_sink sink, void*
   if (nl == 1) {
     rc = drain_shard(g, batch_id, 0, sink, user, &st);
   } else {
+    // A batch the output pool refused on some shard goes to the sink from no shard: the recovery
+    // (release older batches, pcdn_retry_batch, drain again) then hands every shard's share over once.
+    for (uint32_t li = 0; li < nl && !rc; li++) {
+      pcdn_batch_result res{};
+      rc = pcdn_poll_shard(e, batch_id, li, &res, 1);
+      if (!rc && res.status == (uint32_t)(-PCDN_EAGAIN))
+        rc = fail(PCDN_EAGAIN, "the batch was refused for space in the output pool: release older batches, pcdn_retry_batch, drain again");
+    }
     // every GPU has its own PCIe link: the shards drain side by side
     std::vector<pcdn_egress_stats> ps(nl);
     std::vector<int> rcs(nl, 0);
     std::vector<std::string> errs(nl);
     std::vector<std::thread> th;
-    for (uint32_t li = 0; li < nl; li++)
+    for (uint32_t li = 0; li < nl && !rc; li++)
       th.emplace_back([&, li] { rcs[li] = drain_shard(g, batch_id, li, sink, user, &ps[li]); if (rcs[li]) errs[li] = pcdn_last_error(); });
     for (auto& t : th) t.join();
     for (uint32_t li = 0; li < nl; li++) {

@@ -126,8 +126,11 @@ static constexpr unsigned long long kOverlapMaxBytes = 3ull << 29;
 static constexpr uint32_t kTimelineBatches = 64;
 
 // run the kernel pipeline of one shard for slot `si`, whose BatchIn is ready (or will be, once
-// ev_ingest fires) in that shard's memory
-int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_direct, bool devparse, bool wait_ingest, bool unblock = false) {
+// ev_ingest fires) in that shard's memory.
+// retry (output pool): the slot holds a batch the pool refused.  Its routing (parse, direct lookup,
+// match, plan: everything that reads the tables) is kept as it was computed at launch; only the passes
+// that place it in the pool and pack it run again: offsets (+ pool finish) and pack.
+int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_direct, bool devparse, bool wait_ingest, bool retry = false) {
   DeviceGuard dg(sh.device);
   ShardSlot& s = sh.slots[si];
   // Default: the pack runs on the main stream.  A/B switch (pack_variant bit 3): run it on the
@@ -171,12 +174,14 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   }
   s.polled = false;
   s.n_msg_errors = 0;
-  if (++s.w.stamp == 0) s.w.stamp = 1;  // validity stamp of this batch's direct buckets / look-back words
-  if (sh.dev.pool && (s.w.stamp & 0x3FFFFFFFu) == 0) {   // the look-back words carry 30 bits of it
+  // validity stamp of this batch's direct buckets / look-back words (a retry keeps it: the fused
+  // kernel's direct bounds of the first run are valid under it)
+  if (!retry && ++s.w.stamp == 0) s.w.stamp = 1;
+  if (!retry && sh.dev.pool && (s.w.stamp & 0x3FFFFFFFu) == 0) {   // the look-back words carry 30 bits of it
     s.w.stamp++;
     CUDA_TRY(cudaMemsetAsync(s.w.lb_state, 0, ((size_t)sh.dev.N / 256 + 1) * 8, st));
   }
-  s.w.pool_unblock = unblock ? 1u : 0u;
+  s.w.pool_unblock = retry ? 1u : 0u;
   // latency path of the smallest geometry: match + plan + offsets in one cluster launch that also
   // zeroes / publishes the counters (kernels.cu: k_ctrl_small)
   // (one cluster of 8 CTAs: worth it while the whole match is a few passes — a 128-message batch on a
@@ -191,20 +196,24 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   if (sh.dev.pool && !fused) s.spans_mapped = false;   // k_pool_finish patches the table: keep it in HBM until it is final
   s.w.spans = s.spans_mapped ? s.d_spans_map : s.d_spans_dev;
   s.w.overflow = s.spans_mapped ? s.d_ovf_map : s.d_ovf_dev;
-  const bool zero_in_kernel = fused && !devparse;  // (k_parse counts into the batch counters before the fused kernel)
+  const bool zero_in_kernel = fused && !devparse && !retry;  // (k_parse counts into the batch counters before the fused kernel)
   if (timed) CUDA_TRY(cudaEventRecord(tev[0], st));
-  if (!zero_in_kernel) launch_batch_begin(sh.dev, s.w, s.in, has_direct, st);
-  if (devparse) launch_parse(sh.dev, s.w, s.in, st);
-  if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
+  if (retry) {
+    launch_pool_retry_begin(sh.dev, s.w, st);
+  } else {
+    if (!zero_in_kernel) launch_batch_begin(sh.dev, s.w, s.in, has_direct, st);
+    if (devparse) launch_parse(sh.dev, s.w, s.in, st);
+    if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
+  }
   if (timed) CUDA_TRY(cudaEventRecord(tev[1], st));
   if (fused) {
-    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, zero_in_kernel, s.d_stats_pub, st);
+    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, zero_in_kernel, s.d_stats_pub, retry, st);
     if (timed) { CUDA_TRY(cudaEventRecord(tev[2], st)); CUDA_TRY(cudaEventRecord(tev[3], st)); }
   } else {
-    launch_match(sh.dev, s.w, s.in, st);
+    if (!retry) launch_match(sh.dev, s.w, s.in, st);
     if (timed) CUDA_TRY(cudaEventRecord(tev[2], st));
-    launch_plan(sh.dev, s.w, s.in, st);
-    launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);
+    if (!retry) launch_plan(sh.dev, s.w, s.in, st);
+    launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);   // pool mode: a pure function of the scratch
     if (timed) CUDA_TRY(cudaEventRecord(tev[3], st));
   }
   if (!s.spans_mapped) {
@@ -1743,8 +1752,7 @@ int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id) {
   if (e->inflight.empty() || e->inflight.front() != batch_id)
     return fail(PCDN_EINVAL, "only the oldest unreleased batch can be retried (release the older ones first)");
   Slot& s = e->slots[si];
-  int rc = flush_journal(e);
-  if (rc) return rc;
+  int rc = 0;
   uint32_t n = 0;
   for (Shard& sh : e->shards) {
     ShardSlot& ss = sh.slots[si];

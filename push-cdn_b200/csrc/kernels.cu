@@ -890,9 +890,11 @@ void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// offsets_only: the retry of a batch the output pool refused — the routing of the first run (direct
+// bounds, match words, plan) is still in the scratch, only the offsets pass runs again.
 template <bool HAS_DIRECT>
 __global__ void __cluster_dims__(8, 1, 1) __launch_bounds__(1024, 1)
-k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish) {
+k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish, int offsets_only) {
   __shared__ uint32_t sm[33];
   __shared__ uint32_t gbase[5];
   const uint32_t tid = threadIdx.x, rank = blockIdx.x;  // grid = one cluster
@@ -900,7 +902,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish)
 
   // ---- direct messages (= k_direct_lookup + the grouping by connection) on CTA 0; at most
   //      kSmallCtrlMsgs of them, so the (connection, message) order is a rank count
-  if (HAS_DIRECT && rank == 0) {
+  if (HAS_DIRECT && rank == 0 && !offsets_only) {
     __shared__ uint32_t skey_s[kSmallCtrlMsgs], sorted_s[kSmallCtrlMsgs];
     __syncthreads();  // counters are zero before the lookup counts dropped messages
     for (uint32_t g0 = 0; g0 < b.n_msgs * 8; g0 += 1024) direct_lookup_body<false>(s, b, w, g0 + tid);  // 128 messages per pass
@@ -924,7 +926,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish)
   }
 
   // ---- match (= k_match): four (message, 256-word block) items per pass and CTA
-  {
+  if (!offsets_only) {
     const uint32_t q = tid >> 8, wl = tid & 255u, nitems = b.n_bcast * s.nblk;
     for (uint32_t i0 = rank * 4; i0 < nitems; i0 += 32) {  // trip count is uniform inside a CTA
       const uint32_t it = i0 + q;
@@ -947,7 +949,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish)
   cluster_sync_all();
 
   // ---- block bases and D_m of every broadcast (thread = message; at most 8 blocks each) on CTA 0
-  if (rank == 0) {
+  if (rank == 0 && !offsets_only) {
     if (tid < b.n_bcast) {
       uint32_t carry = 0;
       for (uint32_t blk = 0; blk < s.nblk; blk++) {
@@ -962,7 +964,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish)
   }
 
   // ---- plan (= the single-block case of k_plan_a) on CTA 0
-  if (rank == 0) {
+  if (rank == 0 && !offsets_only) {
     const uint32_t m = tid;
     const bool valid = m < b.n_msgs;
     const uint32_t d = valid ? w.D[m] : 0;
@@ -1002,9 +1004,23 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish)
   }
 }
 void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool zero_stats,
-                       BatchStats* publish, cudaStream_t st) {
-  if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish);
-  else PCDN_COUNT_LAUNCH, k_ctrl_small<false><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish);
+                       BatchStats* publish, bool offsets_only, cudaStream_t st) {
+  if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish, offsets_only ? 1 : 0);
+  else PCDN_COUNT_LAUNCH, k_ctrl_small<false><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish, offsets_only ? 1 : 0);
+}
+
+// Pool mode, retry of a refused batch: the offsets pass runs again from the counters as the plan left
+// them (no refusal, nothing added yet by the offsets pass, whose counters are atomic sums; pack cursors
+// at 0), and with cleared look-back words, so the fused kernel's look-back waits for this run's totals.
+__global__ void k_pool_retry_begin(BatchStats* bs) {
+  bs->status = 0;
+  bs->n_deliveries = 0; bs->bytes_out = 0;
+  bs->n_spans = 0; bs->n_runs = 0; bs->n_overflow = 0;
+  bs->tile_cursor = 0; bs->cm_cursor = 0;
+}
+void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st) {
+  cudaMemsetAsync(w.lb_state, 0, ((size_t)s.N / 256 + 1) * 8, st);
+  PCDN_COUNT_LAUNCH, k_pool_retry_begin<<<1, 1, 0, st>>>(w.stats);
 }
 
 // where a record goes: `off` units into the connection's own ring, or (pool mode) into the

@@ -212,7 +212,9 @@ void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_
 void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st);
 // fused match + plan + offsets for N <= kSmallCtrlConns and n_msgs <= kSmallCtrlMsgs (one cluster launch)
 void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool zero_stats,
-                       BatchStats* publish, cudaStream_t st);
+                       BatchStats* publish, bool offsets_only, cudaStream_t st);
+// pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
+void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);
 void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t variant, int n_sms, cudaStream_t st);
 void launch_release(const DevState& s, const uint32_t* batch_units, const BatchStats* stats, cudaStream_t st);
 void launch_pool_init(const DevState& s, cudaStream_t st);

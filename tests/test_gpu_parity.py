@@ -164,7 +164,7 @@ def shard_cfg(pcdn, variant):
 
 
 @pytest.mark.parametrize("variant", [0, 4, 2, 8 + 65536, "staged", "runs", "runs-staged", "pool", "pool-st", "pool-staged-runs", "pool-host", "pool-shards", "pool-shards-nccl",
-                                     "host", "host-st", "shards-host", "shards-nccl"])
+                                     "pool-shards-staged", "host", "host-st", "shards-host", "shards-host-staged", "shards-nccl"])
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_random_mixed_batches(pcdn, seed, variant):
     """users + peer brokers, multi-topic broadcasts (fat and thin recipient sets), directs to local,
@@ -172,7 +172,8 @@ def test_random_mixed_batches(pcdn, seed, variant):
     Small engines publish spans straight into mapped host memory; "staged" forces the span path of
     large engines (table in HBM, copied out while the pack runs) on the same workload.
     The 'shards-*' variants run the SAME workload on ONE engine whose connections are spread over
-    several shards (pcdn_config.devices) and compare with the same single unsharded oracle."""
+    several shards (pcdn_config.devices) and compare with the same single unsharded oracle; the
+    '*-staged' ones force the regular control kernels there, so they run with conn_base != 0."""
     rng = random.Random(seed)
     if variant == "staged":
         w = World(pcdn, flags=pcdn.FLAG_STAGED_SPANS, ring_bytes_per_conn=1 << 20)
@@ -187,8 +188,10 @@ def test_random_mixed_batches(pcdn, seed, variant):
             fl |= pcdn.FLAG_STAGED_SPANS | pcdn.FLAG_SPAN_RUNS
         if variant == "pool-host":
             fl |= pcdn.FLAG_HOST_RINGS
-        if variant == "pool-shards":
+        if variant in ("pool-shards", "pool-shards-staged"):
             kw.update(shard_cfg(pcdn, "shards-host"), max_conns=1024)
+        if variant == "pool-shards-staged":
+            fl |= pcdn.FLAG_STAGED_SPANS
         if variant == "pool-shards-nccl":   # every GPU its own pool, batches replicated by the library's ncclBroadcast
             kw.update(shard_cfg(pcdn, "shards-nccl"), max_conns=1024)
             fl |= pcdn.FLAG_SPAN_RUNS
@@ -203,7 +206,9 @@ def test_random_mixed_batches(pcdn, seed, variant):
                   ring_bytes_per_conn=1 << 20, max_conns=2048)
         assert w.e.host_rings() != 0
     elif isinstance(variant, str):
-        w = World(pcdn, ring_bytes_per_conn=1 << 20, max_conns=1024, **shard_cfg(pcdn, variant))
+        staged = variant.endswith("-staged")
+        w = World(pcdn, ring_bytes_per_conn=1 << 20, max_conns=1024, flags=pcdn.FLAG_STAGED_SPANS if staged else 0,
+                  **shard_cfg(pcdn, variant.removesuffix("-staged")))
         assert w.e.num_shards()[0] >= 2
     elif variant == 8 + 65536:
         # the pack on its own stream (overlaps the next batch's control kernels), forced onto the
