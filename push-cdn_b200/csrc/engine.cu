@@ -119,6 +119,37 @@ int acquire_open_slot(pcdn_engine* e) {
   return fail(PCDN_EAGAIN, "all batch slots are in flight: poll and release a batch first");
 }
 
+// drop the open batch (nothing of it has been launched) and give its permits back
+void abandon_open(pcdn_engine* e) {
+  if (e->open_slot < 0) return;
+  Slot& s = e->slots[e->open_slot];
+  e->inflight_bytes -= std::min(e->inflight_bytes, s.ingress_bytes);
+  e->stats.bytes_in -= std::min(e->stats.bytes_in, s.ingress_bytes);
+  slot_reset_open(s);
+  s.state = SLOT_FREE;
+  e->open_slot = -1;
+}
+
+// Descriptor block of a batch: its per-message arrays at these offsets from the block's base (host-staged
+// batches, and device-resident ones as sharded engines replicate them)
+struct DescLayout {
+  uint32_t n_msgs, n_bcast;
+  size_t o_kind, o_flags, o_slot, o_len, o_aoff, o_alen, o_bidx, o_top, total;
+  DescLayout(uint32_t n, uint32_t nb, size_t n_topics) : n_msgs(n), n_bcast(nb) {
+    o_kind = 0; o_flags = align_up(o_kind + n, 16); o_slot = align_up(o_flags + n, 16);
+    o_len = o_slot + (size_t)n * 4; o_aoff = o_len + (size_t)n * 4; o_alen = o_aoff + (size_t)n * 4;
+    o_bidx = o_alen + (size_t)n * 4; o_top = align_up(o_bidx + (size_t)nb * 4, 16);
+    total = align_up(o_top + n_topics * 2, 16);
+  }
+};
+
+// the kernels' view of a batch whose frames lie at `arena` and whose descriptor block lies at `desc`
+BatchIn bind_batch(const uint8_t* arena, const uint8_t* desc, const DescLayout& L) {
+  return BatchIn{L.n_msgs, L.n_bcast, arena, desc + L.o_kind, desc + L.o_flags, (const uint32_t*)(desc + L.o_slot),
+                 (const uint32_t*)(desc + L.o_len), (const uint32_t*)(desc + L.o_aoff), (const uint32_t*)(desc + L.o_alen),
+                 (const uint16_t*)(desc + L.o_top), (const uint32_t*)(desc + L.o_bidx)};
+}
+
 // The adaptive pack-stream overlap applies to batches whose previous output was at most this many bytes.
 // With every step queued ahead, overlapped packs can lose the launch race against the next control stage
 // and run much longer; the overlap hides at most the short control stage, so it stops paying for long packs.
@@ -243,11 +274,11 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   return 0;
 }
 
-// every local shard runs the pipeline; the slot becomes the newest in-flight batch
-int launch_pipeline(pcdn_engine* e, uint32_t si, uint32_t n_direct, bool wait_ingest) {
+// every local shard runs the pipeline on the open slot `si`; it becomes the newest in-flight batch
+int launch_pipeline(pcdn_engine* e, uint32_t si, bool wait_ingest) {
   Slot& s = e->slots[si];
   for (Shard& sh : e->shards) {
-    int rc = launch_shard_pipeline(e, sh, si, n_direct, s.devparse, wait_ingest);
+    int rc = launch_shard_pipeline(e, sh, si, s.n_direct, s.devparse, wait_ingest);
     if (rc) return rc;
   }
   s.state = SLOT_INFLIGHT;
@@ -255,6 +286,9 @@ int launch_pipeline(pcdn_engine* e, uint32_t si, uint32_t n_direct, bool wait_in
   s.batch_id = e->next_batch_id++;
   s.counted = false;
   e->inflight.push_back(s.batch_id);
+  e->open_slot = -1;
+  e->stats.batches++;
+  e->stats.msgs += s.n_msgs;
   return 0;
 }
 
@@ -365,67 +399,46 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
   const uint32_t si = (uint32_t)e->open_slot;
   Slot& s = e->slots[si];
   const uint32_t n = (uint32_t)s.kind.size();
-  if (n == 0) { s.state = SLOT_FREE; e->open_slot = -1; return 0; }
+  if (n == 0) { abandon_open(e); return 0; }
   if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
   int rc = flush_journal(e);
   if (rc) return rc;
-  // descriptor block layout (offsets 16-byte aligned)
-  size_t o_kind = 0, o_flags = align_up(o_kind + n, 16), o_slot = align_up(o_flags + n, 16);
-  size_t o_len = o_slot + (size_t)n * 4, o_aoff = o_len + (size_t)n * 4, o_alen = o_aoff + (size_t)n * 4;
-  size_t o_bidx = o_alen + (size_t)n * 4, o_top = align_up(o_bidx + s.bcast_index.size() * 4, 16);
-  size_t total = align_up(o_top + s.topics.size() * 2, 16);
-  if (total > e->desc_cap) return fail(PCDN_ENOSPC, "descriptor block overflow");
+  const DescLayout L(n, (uint32_t)s.bcast_index.size(), s.topics.size());   // fits desc_cap (checked at create)
   // Small batches ride in ONE host→device copy: the descriptor block is appended to the frame arena
   // when it fits there (one DMA + one API call less on the latency path); otherwise two copies.
   // Sharded engines always use the appended layout: the batch is one ingest region.
   const size_t doff = align_up(s.arena_used, 256);
-  const bool one_copy = e->sharded || (doff + total <= (size_t)e->cfg.max_batch_bytes + 64 && doff + total <= (64u << 10));
+  const bool one_copy = e->sharded || (doff + L.total <= (size_t)e->cfg.max_batch_bytes + 64 && doff + L.total <= (64u << 10));
   uint8_t* hd = one_copy ? s.h_arena + doff : s.h_desc;
-  std::memcpy(hd + o_kind, s.kind.data(), n);
-  std::memcpy(hd + o_flags, s.flags.data(), n);
-  std::memcpy(hd + o_slot, s.slot_off16.data(), (size_t)n * 4);
-  std::memcpy(hd + o_len, s.raw_len.data(), (size_t)n * 4);
-  std::memcpy(hd + o_aoff, s.aux_off.data(), (size_t)n * 4);
-  std::memcpy(hd + o_alen, s.aux_len.data(), (size_t)n * 4);
-  if (!s.bcast_index.empty()) std::memcpy(hd + o_bidx, s.bcast_index.data(), s.bcast_index.size() * 4);
-  if (!s.topics.empty()) std::memcpy(hd + o_top, s.topics.data(), s.topics.size() * 2);
+  std::memcpy(hd + L.o_kind, s.kind.data(), n);
+  std::memcpy(hd + L.o_flags, s.flags.data(), n);
+  std::memcpy(hd + L.o_slot, s.slot_off16.data(), (size_t)n * 4);
+  std::memcpy(hd + L.o_len, s.raw_len.data(), (size_t)n * 4);
+  std::memcpy(hd + L.o_aoff, s.aux_off.data(), (size_t)n * 4);
+  std::memcpy(hd + L.o_alen, s.aux_len.data(), (size_t)n * 4);
+  if (!s.bcast_index.empty()) std::memcpy(hd + L.o_bidx, s.bcast_index.data(), s.bcast_index.size() * 4);
+  if (!s.topics.empty()) std::memcpy(hd + L.o_top, s.topics.data(), s.topics.size() * 2);
   if (e->sharded) {
     std::memset(s.h_arena + s.arena_used, 0, doff - s.arena_used);
-    if ((rc = ingest_staged(e, si, s.h_arena, doff + total))) return rc;
+    if ((rc = ingest_staged(e, si, s.h_arena, doff + L.total))) return rc;
   } else {
     Shard& sh = e->shards[0];
     DeviceGuard dg(sh.device);
     ShardSlot& ss = sh.slots[si];
     if (one_copy) {
-      CUDA_TRY(cudaMemcpyAsync(ss.d_arena, s.h_arena, doff + total, cudaMemcpyHostToDevice, sh.stream));
+      CUDA_TRY(cudaMemcpyAsync(ss.d_arena, s.h_arena, doff + L.total, cudaMemcpyHostToDevice, sh.stream));
     } else {
       CUDA_TRY(cudaMemcpyAsync(ss.d_arena, s.h_arena, align_up(s.arena_used, 16), cudaMemcpyHostToDevice, sh.stream));
-      CUDA_TRY(cudaMemcpyAsync(ss.d_desc, s.h_desc, total, cudaMemcpyHostToDevice, sh.stream));
+      CUDA_TRY(cudaMemcpyAsync(ss.d_desc, s.h_desc, L.total, cudaMemcpyHostToDevice, sh.stream));
     }
   }
   for (Shard& sh : e->shards) {
     ShardSlot& ss = sh.slots[si];
-    uint8_t* dd = one_copy ? ss.d_arena + doff : ss.d_desc;
-    ss.in.n_msgs = n;
-    ss.in.n_bcast = (uint32_t)s.bcast_index.size();
-    ss.in.arena = ss.d_arena;
-    ss.in.kind = dd + o_kind;
-    ss.in.flags = dd + o_flags;
-    ss.in.slot_off16 = (const uint32_t*)(dd + o_slot);
-    ss.in.raw_len = (const uint32_t*)(dd + o_len);
-    ss.in.aux_off = (const uint32_t*)(dd + o_aoff);
-    ss.in.aux_len = (const uint32_t*)(dd + o_alen);
-    ss.in.bcast_index = (const uint32_t*)(dd + o_bidx);
-    ss.in.topics = (const uint16_t*)(dd + o_top);
+    ss.in = bind_batch(ss.d_arena, one_copy ? ss.d_arena + doff : ss.d_desc, L);
   }
-  s.device_input = false;
   s.n_msgs = n;
-  rc = launch_pipeline(e, si, s.n_direct, e->sharded);
-  if (rc) return rc;
+  if ((rc = launch_pipeline(e, si, e->sharded))) return rc;
   if (batch_id) *batch_id = s.batch_id;
-  e->open_slot = -1;
-  e->stats.batches++;
-  e->stats.msgs += n;
   return 0;
 }
 
@@ -439,77 +452,139 @@ int before_state_change(pcdn_engine* e) {
   return rc;
 }
 
-// append one message to the open batch (flushing a full batch first)
-int append_msg(pcdn_engine* e, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
-               const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw, uint32_t raw_len) {
-  if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
-  if (raw_len > 0x1FFFFFFFu) return fail(PCDN_EINVAL, "message larger than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25)");
-  if (kind != PCDN_KIND_BROADCAST && kind != PCDN_KIND_DIRECT) return fail(PCDN_EINVAL, "kind must be broadcast or direct");
+// One message on its way into a batch (an aggregate: InMsg{} is the empty message).
+struct InMsg {
+  uint8_t kind, flags;
+  bool prune;                        // broadcast: apply Topic::prune to the wire topic list
+  uint32_t raw_len, key_len;         // key_len: direct message's recipient length (0 = no recipient)
+  uint32_t n_listed, n_topics;       // broadcast: entries of the topic list below, entries it adds to the batch
+  const uint8_t* raw;
+  const uint8_t* key;                // direct: the recipient
+  const uint16_t* topic_ids;         // broadcast: the topic ids (API calls), or null and
+  const uint8_t* wire_topics;        // a frame's wire topic list, pruned or verbatim
+};
+
+// What one message adds to a batch: a 16-byte frame slot (4-byte length hole, raw bytes, zero pad),
+// `key_bytes` of recipient key staged beside it (0 when the key is read in place) and topic entries.
+struct MsgShape {
+  uint8_t kind;
+  uint32_t raw_len, key_bytes, n_topics;
+  size_t bytes() const { return align_up(4 + (size_t)raw_len, 16) + key_bytes; }
+};
+
+// What a batch holds.  `ingress`: bytes admitted to it that e->inflight_bytes does not count yet.
+struct BatchFill {
+  uint32_t msgs = 0, bcast = 0;
+  uint64_t bytes = 0, topics = 0, ingress = 0;
+  void add(const MsgShape& m) {
+    msgs++; bcast += m.kind == PCDN_KIND_BROADCAST ? 1 : 0;
+    bytes += m.bytes(); topics += m.n_topics; ingress += m.raw_len;
+  }
+};
+BatchFill fill_of(const Slot& s) { return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0}; }
+
+// The per-batch limits: nullptr when `m` still fits a batch that holds `f`, else the limit it would
+// break.  A message that does not fit an empty batch (BatchFill{}) never fits.
+const char* batch_limit(const pcdn_engine* e, const BatchFill& f, const MsgShape& m) {
   const pcdn_config& c = e->cfg;
-  if (c.global_memory_pool_size) {
-    // limiter/mod.rs:56-68: the frame's length in permits must be available before it is accepted
-    if (raw_len > c.global_memory_pool_size) return fail(PCDN_EINVAL, "message larger than the global memory pool");
-    if (e->inflight_bytes + raw_len > c.global_memory_pool_size)
-      return fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
-  }
-  const size_t slot_bytes = align_up(4 + (size_t)raw_len, 16);
-  size_t need = slot_bytes + (kind == PCDN_KIND_DIRECT ? align_up(recipient_len, 16) : 0);
-  if (need + 64 > c.max_batch_bytes) return fail(PCDN_ENOSPC, "message does not fit max_batch_bytes");
-  if (kind == PCDN_KIND_DIRECT && recipient_len > c.max_key_len) {
-    // longer than any key in the table: cannot match (bytewise identity, R8) → dropped silently,
-    // but batch order bookkeeping still wants the message; route it as "no recipient"
-    recipient_len = 0;
-  }
-  for (int attempt = 0; attempt < 2; attempt++) {
-    int rc = acquire_open_slot(e);
-    if (rc) return rc;
-    Slot& s = e->slots[e->open_slot];
-    bool full = s.kind.size() >= c.max_batch_msgs || s.arena_used + need + 64 > c.max_batch_bytes ||
-                (kind == PCDN_KIND_BROADCAST && s.bcast_index.size() >= c.max_batch_bcast) ||
-                s.topics.size() + n_topics > e->topics_cap;
-    if (!full) break;
-    if (attempt == 1) return fail(PCDN_ENOSPC, "message does not fit an empty batch");
-    if ((rc = flush_open(e, nullptr))) return rc;
-  }
-  Slot& s = e->slots[e->open_slot];
-  const uint32_t m = (uint32_t)s.kind.size();
-  const size_t off = s.arena_used;  // 16-byte aligned
+  if (f.msgs >= c.max_batch_msgs) return "max_batch_msgs";
+  if (f.bytes + m.bytes() + 64 > c.max_batch_bytes) return "max_batch_bytes";
+  if (m.kind == PCDN_KIND_BROADCAST && f.bcast >= c.max_batch_bcast) return "max_batch_bcast";
+  if (f.topics + m.n_topics > e->topics_cap) return "the topic entries of the descriptor block";
+  return nullptr;
+}
+
+// a frame this engine never accepts (PCDN_EINVAL): the reason, else nullptr
+const char* msg_invalid(const pcdn_engine* e, uint32_t raw_len) {
+  if (raw_len > 0x1FFFFFFFu) return "message larger than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25)";
+  if (e->cfg.global_memory_pool_size && raw_len > e->cfg.global_memory_pool_size) return "message larger than the global memory pool";
+  return nullptr;
+}
+
+// limiter/mod.rs:56-68: the frames' length in permits must be available before they are accepted
+bool pool_admits(const pcdn_engine* e, uint64_t bytes) {
+  return !e->cfg.global_memory_pool_size || e->inflight_bytes + bytes <= e->cfg.global_memory_pool_size;
+}
+
+// A recipient longer than any key in the table cannot match (bytewise identity, R8): the message is
+// dropped, but batch order bookkeeping still wants it, so it is routed as "no recipient".
+uint32_t routed_key_len(const pcdn_engine* e, uint32_t len) { return len > e->cfg.max_key_len ? 0 : len; }
+
+// a message of the C ABI's handle / submit calls
+InMsg api_msg(const pcdn_engine* e, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
+              const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw, uint32_t raw_len) {
+  InMsg m{};
+  m.kind = kind; m.flags = flags; m.raw = raw; m.raw_len = raw_len;
+  if (kind == PCDN_KIND_DIRECT) { m.key = recipient; m.key_len = routed_key_len(e, recipient_len); }
+  else { m.topic_ids = topics; m.n_listed = m.n_topics = n_topics; }
+  return m;
+}
+
+void slot_resize(Slot& s, const BatchFill& f) {
+  s.kind.resize(f.msgs); s.flags.resize(f.msgs); s.slot_off16.resize(f.msgs); s.raw_len.resize(f.msgs);
+  s.aux_off.resize(f.msgs); s.aux_len.resize(f.msgs); s.bcast_index.resize(f.bcast); s.topics.resize(f.topics);
+}
+
+// Write message `mi` of slot `s`: its frame into the slot at arena offset `off` and its descriptor
+// entries (the arrays are sized already).  `aux_off`: a direct message's key offset in the arena (the
+// caller placed the key), a broadcast's first entry in s.topics; `bcast_pos`: a broadcast's place in
+// bcast_index.  It touches only what message mi owns, so threads may write distinct messages at once.
+void write_msg(Slot& s, uint32_t mi, size_t off, uint32_t aux_off, uint32_t bcast_pos, const InMsg& m, uint32_t n_valid) {
   uint8_t* dst = s.h_arena + off;
   std::memset(dst, 0, 4);
-  if (raw_len) std::memcpy(dst + 4, raw, raw_len);
-  std::memset(dst + 4 + raw_len, 0, slot_bytes - 4 - raw_len);
-  s.arena_used += slot_bytes;
-  s.kind.push_back(kind);
-  s.flags.push_back(flags);
-  s.slot_off16.push_back((uint32_t)(off / 16));
-  s.raw_len.push_back(raw_len);
-  s.ingress_bytes += raw_len;
-  e->inflight_bytes += raw_len;
-  e->stats.bytes_in += raw_len;
-  if (kind == PCDN_KIND_BROADCAST) {
-    s.aux_off.push_back((uint32_t)s.topics.size());
-    s.aux_len.push_back(n_topics);
-    for (uint32_t i = 0; i < n_topics; i++) s.topics.push_back(topics[i]);
-    s.bcast_index.push_back(m);
-  } else {
+  if (m.raw_len) std::memcpy(dst + 4, m.raw, m.raw_len);
+  std::memset(dst + 4 + m.raw_len, 0, align_up(4 + (size_t)m.raw_len, 16) - 4 - m.raw_len);
+  s.kind[mi] = m.kind; s.flags[mi] = m.flags; s.slot_off16[mi] = (uint32_t)(off / 16); s.raw_len[mi] = m.raw_len;
+  s.aux_off[mi] = aux_off;
+  if (m.kind == PCDN_KIND_DIRECT) { s.aux_len[mi] = m.key_len; return; }
+  s.aux_len[mi] = m.n_topics;
+  s.bcast_index[bcast_pos] = mi;
+  for (uint32_t t = 0, k = aux_off; t < m.n_listed; t++) {
+    if (m.topic_ids) s.topics[k++] = m.topic_ids[t];
+    else if (!m.prune || topic_kept(m.wire_topics, t, n_valid)) s.topics[k++] = m.wire_topics[t];
+  }
+}
+
+// the open slot `s` now holds `f`: messages up to f.msgs are written
+void slot_commit(pcdn_engine* e, Slot& s, const BatchFill& f, bool devparse) {
+  s.arena_used = f.bytes; s.n_direct = f.msgs - f.bcast; s.devparse |= devparse;
+  s.ingress_bytes += f.ingress; e->inflight_bytes += f.ingress; e->stats.bytes_in += f.ingress;
+}
+
+// append one message to the open batch (launching a full batch first)
+int append_msg(pcdn_engine* e, const InMsg& m) {
+  if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
+  if (m.kind != PCDN_KIND_BROADCAST && m.kind != PCDN_KIND_DIRECT) return fail(PCDN_EINVAL, "kind must be broadcast or direct");
+  const bool direct = m.kind == PCDN_KIND_DIRECT;
+  MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(m.key_len, 16) : 0u, m.n_topics};  // key staged: the worst case
+  if (const char* why = msg_invalid(e, m.raw_len)) return fail(PCDN_EINVAL, why);
+  if (const char* lim = batch_limit(e, BatchFill{}, shape)) return fail(PCDN_ENOSPC, std::string("message does not fit an empty batch: ") + lim);
+  if (!pool_admits(e, m.raw_len)) return fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
+  int rc = acquire_open_slot(e);
+  if (!rc && batch_limit(e, fill_of(e->slots[e->open_slot]), shape) && !(rc = flush_open(e, nullptr))) rc = acquire_open_slot(e);
+  if (rc) return rc;
+  Slot& s = e->slots[e->open_slot];
+  BatchFill f = fill_of(s);
+  const size_t off = f.bytes;  // 16-byte aligned
+  uint32_t aux_off = (uint32_t)f.topics;
+  if (direct) {
     // recipient key: read it in place when it lies inside the frame at a 4-byte aligned offset
     // (multi-process groups always stage it beside the frame: the layout must not depend on how a
     // process happens to hold the bytes)
-    size_t koff;
-    if (recipient_len && recipient >= raw && recipient + recipient_len <= raw + raw_len &&
-        ((off + 4 + (size_t)(recipient - raw)) & 3) == 0 && e->world_shards == e->shards.size()) {
-      koff = off + 4 + (size_t)(recipient - raw);
+    if (m.key_len && m.key >= m.raw && m.key + m.key_len <= m.raw + m.raw_len &&
+        ((off + 4 + (size_t)(m.key - m.raw)) & 3) == 0 && e->world_shards == e->shards.size()) {
+      aux_off = (uint32_t)(off + 4 + (size_t)(m.key - m.raw));
+      shape.key_bytes = 0;
     } else {
-      koff = s.arena_used;
-      size_t kb = align_up(recipient_len, 16);
-      if (recipient_len) std::memcpy(s.h_arena + koff, recipient, recipient_len);
-      std::memset(s.h_arena + koff + recipient_len, 0, kb - recipient_len);
-      s.arena_used += kb;
+      aux_off = (uint32_t)(off + align_up(4 + (size_t)m.raw_len, 16));
+      if (m.key_len) std::memcpy(s.h_arena + aux_off, m.key, m.key_len);
+      std::memset(s.h_arena + aux_off + m.key_len, 0, shape.key_bytes - m.key_len);
     }
-    s.aux_off.push_back((uint32_t)koff);
-    s.aux_len.push_back(recipient_len);
-    s.n_direct++;
   }
+  f.add(shape);
+  slot_resize(s, f);
+  write_msg(s, f.msgs - 1, off, aux_off, f.bcast - 1, m, e->cfg.n_valid_topics);
+  slot_commit(e, s, f, (m.flags & MSGF_DEVPARSE) != 0);
   return 0;
 }
 
@@ -778,6 +853,8 @@ int init_device(pcdn_engine* e) {
   const uint32_t M = c.max_batch_msgs;
   e->topics_cap = (size_t)M * 4 + 4096;
   e->desc_cap = align_up((size_t)M * 2 + 64, 16) + (size_t)M * 20 + 64 + e->topics_cap * 2 + 64;
+  if (DescLayout(M, std::min(M, c.max_batch_bcast), e->topics_cap).total > e->desc_cap)
+    return fail(PCDN_EINVAL, "the descriptor block of a full batch exceeds desc_cap");
   // sharded engines keep frames + descriptor block in one ingest region (and device-input batches
   // need room for the descriptor arrays behind the frames)
   e->arena_cap = c.max_batch_bytes + 64 + (e->sharded ? 256 + e->desc_cap : 0);
@@ -1075,24 +1152,46 @@ int pcdn_handle_broadcast_message(pcdn_engine* e, const uint16_t* topics, uint32
                                   uint32_t raw_len, int to_users_only) {
   GUARD_BEGIN
   LOCK;
-  return append_msg(e, PCDN_KIND_BROADCAST, to_users_only ? PCDN_TO_USERS_ONLY : 0, topics, n_topics, nullptr, 0, raw, raw_len);
+  return append_msg(e, api_msg(e, PCDN_KIND_BROADCAST, to_users_only ? PCDN_TO_USERS_ONLY : 0, topics, n_topics, nullptr, 0, raw, raw_len));
   GUARD_END
 }
 int pcdn_handle_direct_message(pcdn_engine* e, const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw,
                                uint32_t raw_len, int to_user_only) {
   GUARD_BEGIN
   LOCK;
-  return append_msg(e, PCDN_KIND_DIRECT, to_user_only ? PCDN_TO_USERS_ONLY : 0, nullptr, 0, recipient, recipient_len, raw, raw_len);
+  return append_msg(e, api_msg(e, PCDN_KIND_DIRECT, to_user_only ? PCDN_TO_USERS_ONLY : 0, nullptr, 0, recipient, recipient_len, raw, raw_len));
   GUARD_END
 }
 
-// device-parse mode: Broadcast / Direct frames are only tag-peeked and copied; k_parse does the rest
-static int append_frame_devparse(pcdn_engine* e, int kind, bool from_broker, const uint8_t* raw, uint32_t raw_len) {
-  uint8_t flags = MSGF_DEVPARSE | (from_broker ? MSGF_USERS_ONLY : 0);
-  if (kind == PCDN_KIND_BROADCAST && !from_broker) flags |= MSGF_PRUNE;  // user-origin only (handler.rs:157 vs user/handler.rs:133)
-  int rc = append_msg(e, (uint8_t)kind, flags, nullptr, 0, nullptr, 0, raw, raw_len);
-  if (rc == 0) e->slots[e->open_slot].devparse = true;
-  return rc;
+// ---- frames to messages: user_receive_loop / broker_receive_loop (user/handler.rs, broker/handler.rs) ----
+static constexpr uint32_t kMaxWireTopics = 65536 / 8;
+
+// Device-parse engines without a hook for `origin`: a Direct or Broadcast frame is only tag-peeked
+// and copied; k_parse does the rest.  false: the frame takes the host parse.
+static bool devparse_msg(const pcdn_engine* e, uint32_t origin, const uint8_t* raw, uint32_t raw_len, InMsg* m) {
+  if (!(e->cfg.flags & PCDN_FLAG_DEVICE_PARSE) || e->hook[origin]) return false;
+  const int k = peek_kind_core(raw, raw_len);
+  if (k != PCDN_KIND_DIRECT && k != PCDN_KIND_BROADCAST) return false;
+  *m = InMsg{};
+  m->kind = (uint8_t)k; m->raw = raw; m->raw_len = raw_len;
+  m->flags = MSGF_DEVPARSE | (origin ? MSGF_USERS_ONLY : 0) | (k == PCDN_KIND_BROADCAST && !origin ? MSGF_PRUNE : 0);  // prune: user origin only (handler.rs:157 vs user/handler.rs:133)
+  return true;
+}
+
+// A parsed Direct or Broadcast frame as a message.  `f0` is its field 0 (the recipient or the wire topic
+// list; a hook may have replaced it).  Broker-origin messages go to users only; user-origin topic lists
+// are pruned (Topic::prune, user/handler.rs:133), broker-origin ones kept verbatim (handler.rs:157).
+// 0, or an error code and *why.
+static int parsed_msg(const pcdn_engine* e, uint32_t origin, int kind, const uint8_t* raw, uint32_t raw_len,
+                      const uint8_t* f0, uint32_t f0_len, InMsg* m, const char** why) {
+  *m = InMsg{};
+  m->kind = (uint8_t)kind; m->raw = raw; m->raw_len = raw_len; m->flags = origin ? MSGF_USERS_ONLY : 0;
+  if (kind == PCDN_KIND_DIRECT) { m->key = f0; m->key_len = routed_key_len(e, f0_len); return 0; }
+  if (f0_len > kMaxWireTopics) { *why = "topic list too long"; return PCDN_EPARSE; }
+  m->wire_topics = f0; m->n_listed = f0_len; m->prune = !origin;
+  for (uint32_t t = 0; t < f0_len; t++) m->n_topics += !m->prune || topic_kept(f0, t, e->cfg.n_valid_topics) ? 1u : 0u;
+  if (m->n_topics == 0 && m->prune) { *why = "supplied no valid topics"; return PCDN_EPRUNE; }
+  return 0;
 }
 
 // MessageHookDef::on_message_received on the parsed message (def.rs:79-92).  Returns 0 = process,
@@ -1126,75 +1225,48 @@ static int run_hook(pcdn_engine* e, int origin, const ParsedFrame& pf, const uin
   return 0;
 }
 
-static int user_receive_locked(pcdn_engine* e, const uint8_t* sender_key, uint32_t key_len, const uint8_t* raw, uint32_t raw_len) {
-  if ((e->cfg.flags & PCDN_FLAG_DEVICE_PARSE) && !e->hook[0]) {
-    const int k = peek_kind_core(raw, raw_len);
-    if (k == PCDN_KIND_DIRECT || k == PCDN_KIND_BROADCAST) return append_frame_devparse(e, k, false, raw, raw_len);
-  }
+// One iteration of user_receive_loop (origin 0, `sender` = the user's key) or broker_receive_loop
+// (origin 1, `sender` = the peer's identifier).  A broker-origin frame of another kind returns 1.
+static int receive_locked(pcdn_engine* e, uint32_t origin, const uint8_t* sender, uint32_t sender_len, const uint8_t* raw, uint32_t raw_len) {
+  InMsg m;
+  if (devparse_msg(e, origin, raw, raw_len, &m)) return append_msg(e, m);
   ParsedFrame pf;
   if (!parse_frame(raw, raw_len, &pf)) return fail(PCDN_EPARSE, "failed to deserialize message");
   std::vector<uint8_t> hooked_topics;
   const uint8_t* f0; uint32_t f0_len;
-  int hr = run_hook(e, 0, pf, sender_key, key_len, raw, raw_len, hooked_topics, &f0, &f0_len);
+  int hr = run_hook(e, (int)origin, pf, sender, sender_len, raw, raw_len, hooked_topics, &f0, &f0_len);
   if (hr < 0) return hr;
   if (hr == 1) return 0;  // Ok(HookResult::SkipMessage) => continue
-  uint16_t topics[65536 / 8];
-  switch (pf.kind) {
-    case PCDN_KIND_DIRECT:
-      return append_msg(e, PCDN_KIND_DIRECT, 0, nullptr, 0, f0, f0_len, raw, raw_len);
-    case PCDN_KIND_BROADCAST:
-    case PCDN_KIND_SUBSCRIBE:
-    case PCDN_KIND_UNSUBSCRIBE: {
-      if (f0_len > sizeof(topics) / 2) return fail(PCDN_EPARSE, "topic list too long");
-      uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics);
-      if (n == 0) return fail(PCDN_EPRUNE, "supplied no valid topics");
-      if (pf.kind == PCDN_KIND_BROADCAST) return append_msg(e, PCDN_KIND_BROADCAST, 0, topics, n, nullptr, 0, raw, raw_len);
-      int rc = before_state_change(e);
-      if (rc) return rc;
-      std::string key((const char*)sender_key, key_len);
-      rc = pf.kind == PCDN_KIND_SUBSCRIBE ? e->conns->subscribe_user_to(key, topics, n)
-                                          : e->conns->unsubscribe_user_from(key, topics, n);
-      return rc ? fail(rc, "topic id out of range") : 0;
-    }
-    default:
-      return fail(PCDN_EKIND, "invalid message received");
+  if (pf.kind == PCDN_KIND_DIRECT || pf.kind == PCDN_KIND_BROADCAST) {
+    const char* why = "";
+    const int rc = parsed_msg(e, origin, pf.kind, raw, raw_len, f0, f0_len, &m, &why);
+    return rc ? fail(rc, why) : append_msg(e, m);
   }
-}
-
-static int broker_receive_locked(pcdn_engine* e, const uint8_t* identifier, uint32_t identifier_len, const uint8_t* raw, uint32_t raw_len) {
-  if ((e->cfg.flags & PCDN_FLAG_DEVICE_PARSE) && !e->hook[1]) {
-    const int k = peek_kind_core(raw, raw_len);
-    if (k == PCDN_KIND_DIRECT || k == PCDN_KIND_BROADCAST) return append_frame_devparse(e, k, true, raw, raw_len);
-  }
-  ParsedFrame pf;
-  if (!parse_frame(raw, raw_len, &pf)) return fail(PCDN_EPARSE, "failed to deserialize message");
-  std::vector<uint8_t> hooked_topics;
-  const uint8_t* f0; uint32_t f0_len;
-  int hr = run_hook(e, 1, pf, identifier, identifier_len, raw, raw_len, hooked_topics, &f0, &f0_len);
-  if (hr < 0) return hr;
-  if (hr == 1) return 0;  // Ok(HookResult::SkipMessage) => continue
-  if (pf.kind == PCDN_KIND_DIRECT)
-    return append_msg(e, PCDN_KIND_DIRECT, PCDN_TO_USERS_ONLY, nullptr, 0, f0, f0_len, raw, raw_len);
-  if (pf.kind == PCDN_KIND_BROADCAST) {
-    uint16_t topics[65536 / 8];
-    if (f0_len > sizeof(topics) / 2) return fail(PCDN_EPARSE, "topic list too long");
-    for (uint32_t i = 0; i < f0_len; i++) topics[i] = f0[i];  // broker-origin: no prune (handler.rs:157)
-    return append_msg(e, PCDN_KIND_BROADCAST, PCDN_TO_USERS_ONLY, topics, f0_len, nullptr, 0, raw, raw_len);
-  }
-  return 1;
+  if (origin) return 1;
+  if (pf.kind != PCDN_KIND_SUBSCRIBE && pf.kind != PCDN_KIND_UNSUBSCRIBE) return fail(PCDN_EKIND, "invalid message received");
+  uint16_t topics[kMaxWireTopics];
+  if (f0_len > kMaxWireTopics) return fail(PCDN_EPARSE, "topic list too long");
+  uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics);
+  if (n == 0) return fail(PCDN_EPRUNE, "supplied no valid topics");
+  int rc = before_state_change(e);
+  if (rc) return rc;
+  std::string key((const char*)sender, sender_len);
+  rc = pf.kind == PCDN_KIND_SUBSCRIBE ? e->conns->subscribe_user_to(key, topics, n)
+                                      : e->conns->unsubscribe_user_from(key, topics, n);
+  return rc ? fail(rc, "topic id out of range") : 0;
 }
 
 int pcdn_user_receive(pcdn_engine* e, const uint8_t* sender_key, uint32_t key_len, const uint8_t* raw, uint32_t raw_len) {
   GUARD_BEGIN
   LOCK;
-  return user_receive_locked(e, sender_key, key_len, raw, raw_len);
+  return receive_locked(e, 0, sender_key, key_len, raw, raw_len);
   GUARD_END
 }
 
 int pcdn_broker_receive(pcdn_engine* e, const char* identifier, const uint8_t* raw, uint32_t raw_len) {
   GUARD_BEGIN
   LOCK;
-  return broker_receive_locked(e, (const uint8_t*)identifier, identifier ? (uint32_t)std::strlen(identifier) : 0, raw, raw_len);
+  return receive_locked(e, 1, (const uint8_t*)identifier, identifier ? (uint32_t)std::strlen(identifier) : 0, raw, raw_len);
   GUARD_END
 }
 
@@ -1202,11 +1274,15 @@ int pcdn_broker_receive(pcdn_engine* e, const char* identifier, const uint8_t* r
 extern "C++" {
 namespace {
 
+enum FrameRoute : int8_t { ROUTE_SEQUENTIAL, ROUTE_FAILED, ROUTE_BATCH };
+// what the serial placement scan reads and writes per frame (kept small: the scan streams through it)
 struct FramePlan {
-  int8_t kind;        // 3 / 4 routable; -1 = needs the sequential path (state change, other kinds); -2 = protocol error
+  // ROUTE_SEQUENTIAL: the frame goes through user/broker_receive_locked (state change, other kinds, a
+  // message no batch takes, which reports its error there); ROUTE_FAILED: protocol error `rc`
+  FrameRoute route;
   int32_t rc;
-  uint32_t f0_off, f0_len, ntopics;
-  uint32_t msg_idx, topic_off, bcast_pos;
+  MsgShape shape;
+  uint32_t msg_idx, bcast_pos, topic_off;
   uint64_t arena_off;
 };
 
@@ -1241,130 +1317,79 @@ uint32_t ingest_threads() {
 // run and go through user_receive_locked / broker_receive_locked, so R12 ordering is untouched.
 int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t* rc_out) {
   const pcdn_config& c = e->cfg;
-  const bool dev = (c.flags & PCDN_FLAG_DEVICE_PARSE) != 0;
   const uint32_t T = ingest_threads();
-  if (n < 2048 || T <= 1 || !e->has_device || e->hook[0] || e->hook[1]) {  // a hook sees every parsed message, in order
-    for (uint32_t i = 0; i < n; i++) {
-      const pcdn_frame& f = frames[i];
-      int rc = f.origin ? broker_receive_locked(e, f.sender, f.sender_len, f.raw, f.raw_len) : user_receive_locked(e, f.sender, f.sender_len, f.raw, f.raw_len);
-      if (rc_out) rc_out[i] = rc;
-      if (rc == PCDN_EAGAIN || rc == PCDN_ECUDA || rc == PCDN_ENODEV) return i ? (int)i : rc;
-    }
-    return (int)n;
-  }
-  std::vector<FramePlan> plan(n);
+  // a hook sees every parsed message, in order
+  const bool threaded = n >= 2048 && T > 1 && e->has_device && !e->hook[0] && !e->hook[1];
+  // phase A writes every entry the later phases read
+  std::unique_ptr<FramePlan[]> plan(threaded ? new FramePlan[n] : nullptr);
+  std::unique_ptr<InMsg[]> msgs(threaded ? new InMsg[n] : nullptr);
   // ---- phase A
-  parallel_for(n, T, [&](uint32_t lo, uint32_t hi) {
+  if (threaded) parallel_for(n, T, [&](uint32_t lo, uint32_t hi) {
     for (uint32_t i = lo; i < hi; i++) {
       const pcdn_frame& f = frames[i];
       FramePlan& p = plan[i];
-      p.kind = -1; p.rc = 0; p.f0_off = p.f0_len = p.ntopics = 0;
-      if (f.raw_len > 0x1FFFFFFFu || align_up(4 + (size_t)f.raw_len, 16) + 64 > c.max_batch_bytes ||
-          (c.global_memory_pool_size && f.raw_len > c.global_memory_pool_size)) continue;  // sequential path reports it (PCDN_EINVAL / PCDN_ENOSPC for that frame)
-      if (dev) {
-        const int k = peek_kind_core(f.raw, f.raw_len);
-        if (k == PCDN_KIND_DIRECT || k == PCDN_KIND_BROADCAST) p.kind = (int8_t)k;
-        continue;
+      InMsg& m = msgs[i];
+      const uint32_t origin = f.origin ? 1 : 0;
+      p.route = ROUTE_SEQUENTIAL; p.rc = 0;
+      if (!devparse_msg(e, origin, f.raw, f.raw_len, &m)) {
+        if (c.flags & PCDN_FLAG_DEVICE_PARSE) continue;
+        ParsedFrame pf;
+        const char* why;
+        if (!parse_frame(f.raw, f.raw_len, &pf)) { p.route = ROUTE_FAILED; p.rc = PCDN_EPARSE; continue; }
+        if (pf.kind != PCDN_KIND_DIRECT && pf.kind != PCDN_KIND_BROADCAST) continue;
+        p.rc = parsed_msg(e, origin, pf.kind, f.raw, f.raw_len, f.raw + pf.f0_off, pf.f0_len, &m, &why);
+        if (p.rc) { p.route = ROUTE_FAILED; continue; }
       }
-      ParsedFrame pf;
-      if (!parse_frame(f.raw, f.raw_len, &pf)) { p.kind = -2; p.rc = PCDN_EPARSE; continue; }
-      if (pf.kind == PCDN_KIND_DIRECT) {
-        p.kind = 3; p.f0_off = pf.f0_off; p.f0_len = pf.f0_len > c.max_key_len ? 0 : pf.f0_len;
-      } else if (pf.kind == PCDN_KIND_BROADCAST) {
-        if (pf.f0_len > 8192) { p.kind = -2; p.rc = PCDN_EPARSE; continue; }
-        uint32_t cnt = pf.f0_len;
-        if (!f.origin) {  // user-origin: Topic::prune
-          cnt = 0;
-          for (uint32_t k = 0; k < pf.f0_len; k++) cnt += topic_kept(f.raw + pf.f0_off, k, c.n_valid_topics) ? 1u : 0u;
-          if (cnt == 0) { p.kind = -2; p.rc = PCDN_EPRUNE; continue; }
-        }
-        p.kind = 4; p.f0_off = pf.f0_off; p.f0_len = pf.f0_len; p.ntopics = cnt;
-      }
+      p.shape = MsgShape{m.kind, m.raw_len, 0, m.n_topics};   // the parsed recipient is read in place
+      if (!msg_invalid(e, f.raw_len) && !batch_limit(e, BatchFill{}, p.shape)) p.route = ROUTE_BATCH;
     }
   });
   uint32_t i = 0;
   while (i < n) {
-    FramePlan& p0 = plan[i];
-    if (p0.kind == -2) { if (rc_out) rc_out[i] = p0.rc; i++; continue; }
-    if (p0.kind == -1) {
+    if (!threaded || plan[i].route == ROUTE_SEQUENTIAL) {
       const pcdn_frame& f = frames[i];
-      int rc = f.origin ? broker_receive_locked(e, f.sender, f.sender_len, f.raw, f.raw_len) : user_receive_locked(e, f.sender, f.sender_len, f.raw, f.raw_len);
+      int rc = receive_locked(e, f.origin ? 1 : 0, f.sender, f.sender_len, f.raw, f.raw_len);
       if (rc_out) rc_out[i] = rc;
       if (rc == PCDN_EAGAIN || rc == PCDN_ECUDA || rc == PCDN_ENODEV) return i ? (int)i : rc;
       i++;
       continue;
     }
+    if (plan[i].route == ROUTE_FAILED) { if (rc_out) rc_out[i] = plan[i].rc; i++; continue; }
     // ---- a run of routable frames starting at i: placement scan
     int rc = acquire_open_slot(e);
     if (rc) return i ? (int)i : rc;
     Slot& s = e->slots[e->open_slot];
-    uint32_t nm = (uint32_t)s.kind.size(), nb = (uint32_t)s.bcast_index.size(), nt = (uint32_t)s.topics.size(), nd = 0;
-    uint64_t used = s.arena_used, ingress = 0;
-    const uint32_t m0 = nm, b0 = nb, t0 = nt;
+    BatchFill fill = fill_of(s);
     uint32_t j = i;
     bool full = false;
     for (; j < n; j++) {
       FramePlan& p = plan[j];
-      if (p.kind == -2) continue;
-      if (p.kind == -1) break;
-      const pcdn_frame& f = frames[j];
-      const uint64_t sb = align_up(4 + (size_t)f.raw_len, 16);
-      if (nm >= c.max_batch_msgs || used + sb + 64 > c.max_batch_bytes || (p.kind == 4 && nb >= c.max_batch_bcast) ||
-          (uint64_t)nt + p.ntopics > e->topics_cap) { full = true; break; }
-      if (c.global_memory_pool_size && e->inflight_bytes + ingress + f.raw_len > c.global_memory_pool_size) { full = true; break; }
-      p.msg_idx = nm++; p.arena_off = used; used += sb; ingress += f.raw_len;
-      if (p.kind == 4) { p.bcast_pos = nb++; p.topic_off = nt; nt += dev ? 0 : p.ntopics; }
-      else nd++;
+      if (p.route == ROUTE_FAILED) continue;
+      if (p.route == ROUTE_SEQUENTIAL) break;
+      if (batch_limit(e, fill, p.shape) || !pool_admits(e, fill.ingress + p.shape.raw_len)) { full = true; break; }
+      p.msg_idx = fill.msgs; p.arena_off = fill.bytes; p.bcast_pos = fill.bcast; p.topic_off = (uint32_t)fill.topics;
+      fill.add(p.shape);
     }
     if (j == i) {  // nothing fits: the open batch is full (or the pool is) — launch it and retry, or give up
       if (s.kind.empty()) return i ? (int)i : fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
       if ((rc = flush_open(e, nullptr))) return i ? (int)i : rc;
       continue;
     }
-    // ---- phase B: descriptors by index + raw bytes
-    s.kind.resize(nm); s.flags.resize(nm); s.slot_off16.resize(nm); s.raw_len.resize(nm); s.aux_off.resize(nm); s.aux_len.resize(nm);
-    s.bcast_index.resize(nb); s.topics.resize(nt);
+    // ---- phase B: raw bytes + descriptors by index
+    slot_resize(s, fill);
     parallel_for(j - i, T, [&](uint32_t lo, uint32_t hi) {
       for (uint32_t q = i + lo; q < i + hi; q++) {
         const FramePlan& p = plan[q];
-        if (p.kind < 0) continue;
-        const pcdn_frame& f = frames[q];
-        const uint32_t m = p.msg_idx;
-        const size_t sb = align_up(4 + (size_t)f.raw_len, 16);
-        uint8_t* dst = s.h_arena + p.arena_off;
-        std::memset(dst, 0, 4);
-        if (f.raw_len) std::memcpy(dst + 4, f.raw, f.raw_len);
-        std::memset(dst + 4 + f.raw_len, 0, sb - 4 - f.raw_len);
-        s.kind[m] = (uint8_t)p.kind;
-        uint8_t fl = f.origin ? MSGF_USERS_ONLY : 0;
-        if (dev) fl |= MSGF_DEVPARSE | ((p.kind == 4 && !f.origin) ? MSGF_PRUNE : 0);
-        s.flags[m] = fl;
-        s.slot_off16[m] = (uint32_t)(p.arena_off / 16);
-        s.raw_len[m] = f.raw_len;
-        if (p.kind == 4) {
-          s.bcast_index[p.bcast_pos] = m;
-          s.aux_off[m] = p.topic_off;
-          s.aux_len[m] = dev ? 0 : p.ntopics;
-          if (!dev) {
-            uint32_t k = p.topic_off;
-            for (uint32_t t = 0; t < p.f0_len; t++)
-              if (f.origin || topic_kept(f.raw + p.f0_off, t, c.n_valid_topics)) s.topics[k++] = f.raw[p.f0_off + t];
-          }
-        } else {
-          s.aux_off[m] = dev ? 0 : (uint32_t)(p.arena_off + 4 + p.f0_off);  // recipient read in place (word aligned)
-          s.aux_len[m] = dev ? 0 : p.f0_len;
-        }
+        const InMsg& m = msgs[q];
+        if (p.route != ROUTE_BATCH) continue;
+        const uint32_t aux_off = m.kind == PCDN_KIND_BROADCAST ? p.topic_off
+                                 : m.key ? (uint32_t)(p.arena_off + 4 + (size_t)(m.key - m.raw)) : 0;  // recipient read in place (word aligned)
+        write_msg(s, p.msg_idx, p.arena_off, aux_off, p.bcast_pos, m, c.n_valid_topics);
       }
     });
     if (rc_out)
-      for (uint32_t q = i; q < j; q++) rc_out[q] = plan[q].kind == -2 ? plan[q].rc : 0;
-    s.arena_used = used;
-    s.n_direct += nd;
-    s.ingress_bytes += ingress;
-    e->inflight_bytes += ingress;
-    e->stats.bytes_in += ingress;
-    if (dev && nm > m0) s.devparse = true;
-    (void)b0; (void)t0;
+      for (uint32_t q = i; q < j; q++) rc_out[q] = plan[q].rc;
+    slot_commit(e, s, fill, (c.flags & PCDN_FLAG_DEVICE_PARSE) != 0);
     i = j;
     if (full) {
       if ((rc = flush_open(e, nullptr))) return (int)i;
@@ -1402,47 +1427,34 @@ int pcdn_flush(pcdn_engine* e, uint64_t* batch_id) {
 
 // All-or-nothing check of an explicit batch against every per-batch capacity, BEFORE anything is
 // staged: a refused pcdn_submit leaves no message behind that a later flush would deliver (and a
-// retry would deliver twice).
+// retry would deliver twice).  A dry run of the staging rule over the whole batch, with every
+// recipient key counted as staged beside its frame (the worst case).
 static int validate_explicit_batch(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n) {
   const pcdn_config& c = e->cfg;
   if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
   if (n > c.max_batch_msgs) return fail(PCDN_ENOSPC, "batch larger than max_batch_msgs");
   if (n && !msgs) return fail(PCDN_EINVAL, "null message array");
-  uint64_t bytes = 0, topics = 0, ingress = 0, nb = 0;
+  BatchFill fill;
+  const char* full = nullptr;
   for (uint32_t i = 0; i < n; i++) {
     const pcdn_msg& m = msgs[i];
     if (m.kind != PCDN_KIND_BROADCAST && m.kind != PCDN_KIND_DIRECT)
       return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": kind must be broadcast or direct");
     if (m.flags & ~(uint8_t)PCDN_TO_USERS_ONLY)
       return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": unknown bits in pcdn_msg.flags");
-    if (m.raw_len > 0x1FFFFFFFu) return fail(PCDN_EINVAL, "message larger than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25)");
     if ((m.raw_len && !m.raw) || (m.kind == PCDN_KIND_BROADCAST && m.n_topics && !m.topics) ||
         (m.kind == PCDN_KIND_DIRECT && m.recipient_len && !m.recipient))
       return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": null pointer with non-zero length");
-    if (c.global_memory_pool_size && m.raw_len > c.global_memory_pool_size)
-      return fail(PCDN_EINVAL, "message larger than the global memory pool");
-    bytes += align_up(4 + (size_t)m.raw_len, 16);
-    if (m.kind == PCDN_KIND_DIRECT) bytes += align_up(std::min<uint32_t>(m.recipient_len, c.max_key_len), 16);  // worst case: key staged beside the frame
-    else { nb++; topics += m.n_topics; }
-    ingress += m.raw_len;
+    if (const char* why = msg_invalid(e, m.raw_len)) return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": " + why);
+    const bool direct = m.kind == PCDN_KIND_DIRECT;
+    const MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(std::min<uint32_t>(m.recipient_len, c.max_key_len), 16) : 0u,
+                         direct ? 0u : m.n_topics};
+    if (!full) full = batch_limit(e, fill, shape);
+    fill.add(shape);
   }
-  if (bytes + 64 > c.max_batch_bytes) return fail(PCDN_ENOSPC, "batch does not fit max_batch_bytes");
-  if (nb > c.max_batch_bcast) return fail(PCDN_ENOSPC, "batch has more broadcasts than max_batch_bcast");
-  if (topics > e->topics_cap) return fail(PCDN_ENOSPC, "batch has more topic entries than the descriptor block holds");
-  if (c.global_memory_pool_size && e->inflight_bytes + ingress > c.global_memory_pool_size)
-    return fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
+  if (full) return fail(PCDN_ENOSPC, std::string("batch exceeds ") + full);
+  if (!pool_admits(e, fill.ingress)) return fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
   return 0;
-}
-
-// drop the open batch (nothing of it has been launched) and give its permits back
-static void abandon_open(pcdn_engine* e) {
-  if (e->open_slot < 0) return;
-  Slot& s = e->slots[e->open_slot];
-  e->inflight_bytes -= std::min(e->inflight_bytes, s.ingress_bytes);
-  e->stats.bytes_in -= std::min(e->stats.bytes_in, s.ingress_bytes);
-  slot_reset_open(s);
-  s.state = SLOT_FREE;
-  e->open_slot = -1;
 }
 
 int pcdn_submit(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n, uint64_t* batch_id) {
@@ -1458,7 +1470,7 @@ int pcdn_submit(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n, uint64_t* batc
   for (uint32_t i = 0; i < n; i++) {
     const pcdn_msg& m = msgs[i];
     uint64_t before = e->next_batch_id;
-    rc = append_msg(e, m.kind, m.flags, m.topics, m.n_topics, m.recipient, m.recipient_len, m.raw, m.raw_len);
+    rc = append_msg(e, api_msg(e, m.kind, m.flags, m.topics, m.n_topics, m.recipient, m.recipient_len, m.raw, m.raw_len));
     if (rc == 0 && e->next_batch_id != before) rc = fail(PCDN_ENOSPC, "batch exceeded a per-batch capacity and was split");
     if (rc) { abandon_open(e); return rc; }  // unreachable after validation; never leave a half batch open
   }
@@ -1475,13 +1487,11 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
       b->n_bcast > b->n_msgs)
     return fail(PCDN_EINVAL, "device batch exceeds configured capacities");
   const uint32_t n = b->n_msgs, nb = b->n_bcast;
-  // region layout of the batch inside a receiving shard's arena (sharded engines)
-  const size_t o_arena = 0, o_kind = align_up(b->arena_bytes, 256), o_flags = align_up(o_kind + n, 16), o_slot = align_up(o_flags + n, 16);
-  const size_t o_len = o_slot + (size_t)n * 4, o_aoff = o_len + (size_t)n * 4, o_alen = o_aoff + (size_t)n * 4;
-  const size_t o_bidx = o_alen + (size_t)n * 4, o_top = align_up(o_bidx + (size_t)nb * 4, 16);
-  const size_t total = align_up(o_top + (size_t)b->n_topics_total * 2, 16);
+  // sharded engines: the frames at the start of a receiving shard's arena, the descriptor block behind them
+  const DescLayout L(n, nb, b->n_topics_total);
+  const size_t doff = align_up(b->arena_bytes, 256);
   if (e->sharded) {
-    if (total > e->arena_cap) return fail(PCDN_ENOSPC, "device batch does not fit the shards' ingest region (max_batch_bytes)");
+    if (doff + L.total > e->arena_cap) return fail(PCDN_ENOSPC, "device batch does not fit the shards' ingest region (max_batch_bytes)");
     if (e->ingest == PCDN_INGEST_HOST && e->world_shards != e->shards.size())
       return fail(PCDN_EINVAL, "device-resident batches in a multi-process group need PCDN_INGEST_NCCL");
   }
@@ -1490,8 +1500,7 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
   if ((rc = acquire_open_slot(e))) return rc;
   const uint32_t si = (uint32_t)e->open_slot;
   Slot& s = e->slots[si];
-  auto give_up = [&](int code) { s.state = SLOT_FREE; e->open_slot = -1; return code; };
-  if ((rc = flush_journal(e))) return give_up(rc);
+  if ((rc = flush_journal(e))) { abandon_open(e); return rc; }
   const bool ready = (b->hints & PCDN_BATCH_READY) != 0;
   const bool arena_in_place = b->arena_bytes > (4u << 20);   // large frame arenas are broadcast from the caller's buffer
   if (e->sharded) {
@@ -1504,37 +1513,25 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
       CUDA_TRY(cudaEventRecord(root.ev_submit, root.stream));
     }
     const IngestRegion regs[9] = {
-        {b->arena, o_arena, (size_t)b->arena_bytes}, {b->kind, o_kind, n}, {b->flags, o_flags, n},
-        {b->slot_off16, o_slot, (size_t)n * 4}, {b->raw_len, o_len, (size_t)n * 4}, {b->aux_off, o_aoff, (size_t)n * 4},
-        {b->aux_len, o_alen, (size_t)n * 4}, {b->bcast_index, o_bidx, (size_t)nb * 4}, {b->topics, o_top, (size_t)b->n_topics_total * 2}};
-    if ((rc = ingest_device(e, si, regs, 9, arena_in_place, !ready))) return give_up(rc);
+        {b->arena, 0, (size_t)b->arena_bytes}, {b->kind, doff + L.o_kind, n}, {b->flags, doff + L.o_flags, n},
+        {b->slot_off16, doff + L.o_slot, (size_t)n * 4}, {b->raw_len, doff + L.o_len, (size_t)n * 4},
+        {b->aux_off, doff + L.o_aoff, (size_t)n * 4}, {b->aux_len, doff + L.o_alen, (size_t)n * 4},
+        {b->bcast_index, doff + L.o_bidx, (size_t)nb * 4}, {b->topics, doff + L.o_top, (size_t)b->n_topics_total * 2}};
+    if ((rc = ingest_device(e, si, regs, 9, arena_in_place, !ready))) { abandon_open(e); return rc; }
   }
   for (Shard& sh : e->shards) {
     ShardSlot& ss = sh.slots[si];
-    ss.in.n_msgs = n;
-    ss.in.n_bcast = nb;
-    if (!e->sharded) {  // where the caller put it
-      ss.in.arena = (const uint8_t*)b->arena;
-      ss.in.kind = b->kind; ss.in.flags = b->flags; ss.in.slot_off16 = b->slot_off16; ss.in.raw_len = b->raw_len;
-      ss.in.aux_off = b->aux_off; ss.in.aux_len = b->aux_len; ss.in.topics = b->topics; ss.in.bcast_index = b->bcast_index;
-    } else {            // the replicated copy in this shard's slot region (the root keeps large frames in place)
-      uint8_t* d = ss.d_arena;
-      ss.in.arena = (sh.gindex == 0 && arena_in_place) ? (const uint8_t*)b->arena : d + o_arena;
-      ss.in.kind = d + o_kind; ss.in.flags = d + o_flags;
-      ss.in.slot_off16 = (const uint32_t*)(d + o_slot); ss.in.raw_len = (const uint32_t*)(d + o_len);
-      ss.in.aux_off = (const uint32_t*)(d + o_aoff); ss.in.aux_len = (const uint32_t*)(d + o_alen);
-      ss.in.bcast_index = (const uint32_t*)(d + o_bidx); ss.in.topics = (const uint16_t*)(d + o_top);
-    }
+    if (e->sharded)   // the replicated copy in this shard's slot region (the root keeps large frames in place)
+      ss.in = bind_batch((sh.gindex == 0 && arena_in_place) ? (const uint8_t*)b->arena : ss.d_arena, ss.d_arena + doff, L);
+    else              // where the caller put it
+      ss.in = BatchIn{n, nb, (const uint8_t*)b->arena, b->kind, b->flags, b->slot_off16, b->raw_len, b->aux_off, b->aux_len,
+                      b->topics, b->bcast_index};
   }
   s.device_input = true;
-  s.devparse = false;
   s.n_msgs = n;
-  rc = launch_pipeline(e, si, n - nb, e->sharded);
-  if (rc) return give_up(rc);
+  s.n_direct = n - nb;
+  if ((rc = launch_pipeline(e, si, e->sharded))) { abandon_open(e); return rc; }
   if (batch_id) *batch_id = s.batch_id;
-  e->open_slot = -1;
-  e->stats.batches++;
-  e->stats.msgs += n;
   return 0;
   GUARD_END
 }
@@ -1761,7 +1758,7 @@ int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id) {
       CUDA_TRY(cudaEventSynchronize(ss.ev_done));
     }
     if (ss.h_stats->status != 2) continue;   // this shard packed its share (or refused it for good): leave it alone
-    if ((rc = launch_shard_pipeline(e, sh, (uint32_t)si, s.device_input ? s.n_msgs - ss.in.n_bcast : s.n_direct, s.devparse, false, true))) return rc;
+    if ((rc = launch_shard_pipeline(e, sh, (uint32_t)si, s.n_direct, s.devparse, false, true))) return rc;
     n++;
   }
   if (!n) return fail(PCDN_EINVAL, "the batch was not refused for space");
