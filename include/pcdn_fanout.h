@@ -175,8 +175,25 @@ enum {
    * Span offsets in this mode: pcdn_span.ring_off is in units of PCDN_RECORD_ALIGN (32 B), relative to
    * pcdn_batch_result.pool_base; the bytes are at pool + (pool_base + ring_off) * 32 (pcdn_shard_info:
    * rings_dev / rings_host = the pool).  pcdn_read takes the absolute unit offset pool_base + ring_off. */
-  PCDN_FLAG_OUTPUT_POOL = 16
+  PCDN_FLAG_OUTPUT_POOL = 16,
+  /* Shared-payload delivery: EVERY routed message (broadcast and direct) is delivered by reference.
+   * The payload exists once per batch, in pinned host memory (pcdn_batch_payload), and each delivery is
+   * one 32-byte REFERENCE RECORD in the recipient's ring / the output pool instead of a framed copy (the
+   * reference's fan-out clones a refcounted `Bytes`, it never copies per recipient).  Spans, runs,
+   * n_records, pool_base, wrap, release and retry keep their meaning; bytes_out still counts the 4 + L
+   * wire bytes of each delivery.  Records have no size limit in this mode (one unit each), so messages
+   * far larger than a ring are delivered.  The pack geometry bits of pcdn_config.pack_variant do not
+   * apply (the pack kernel is k_pack_ref).  Record layout (all fields fixed, so bytes compare exactly):
+   *   bytes  0..3   PCDN_REF_MARK (no framed record starts with it: L <= 0x1FFFFFFF)
+   *   bytes  4..7   u32 big-endian L: the 4 wire bytes of the length prefix
+   *   bytes  8..15  u64 little-endian offset of the raw bytes from the batch's payload base
+   *   bytes 16..23  u64 little-endian batch id (resolution is self-checking; a retry writes the same record)
+   *   bytes 24..31  zero
+   * A writer walks a span as usual: at p, if BE32(p) == PCDN_REF_MARK it sends p[4..8) ‖ the L bytes at
+   * payload + offset and advances 32 bytes; otherwise it handles a framed record as before.          */
+  PCDN_FLAG_SHARED_PAYLOAD = 32
 };
+#define PCDN_REF_MARK 0xFFFFFFFFu
 
 /* One routed message.  `raw` is the inbound frame body and is forwarded verbatim (R1). */
 typedef struct pcdn_msg {
@@ -413,7 +430,10 @@ int pcdn_receive_frames(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, in
 int pcdn_flush(pcdn_engine* e, uint64_t* batch_id);
 /* Submit an explicit ordered batch (R9: batch order = per-connection delivery order). */
 int pcdn_submit(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n, uint64_t* batch_id);
-/* Same, inputs already resident in HBM (no host copy, no host parse). */
+/* Same, inputs already resident in HBM (no host copy, no host parse).  PCDN_FLAG_SHARED_PAYLOAD: the
+ * frame arena is copied once into the slot's pinned staging (pcdn_batch_payload) before the batch
+ * runs, and polling the batch waits for that copy; an arena larger than that staging
+ * (max_batch_bytes) is PCDN_ENOSPC. */
 int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* batch, uint64_t* batch_id);
 
 /* ---- data out: replaces Connection::send_message_raw + the per-connection writer task
@@ -423,9 +443,16 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* batch, uint64_t*
 int pcdn_next_batch(pcdn_engine* e, uint64_t* batch_id);
 /* Wait for (block != 0) or test a batch; fills *out (span table is in pinned host memory). */
 int pcdn_poll(pcdn_engine* e, uint64_t batch_id, pcdn_batch_result* out, int block);
-/* Copy `len` ring bytes of a connection to host memory (what a socket writer would send).
+/* Copy `len` ring bytes of a connection to host memory: its records, as a socket writer walks them
+ * (PCDN_FLAG_SHARED_PAYLOAD: reference records, resolved through pcdn_batch_payload).
  * With PCDN_FLAG_HOST_RINGS this is a plain memcpy; prefer pcdn_host_rings() and read in place.  */
 int pcdn_read(pcdn_engine* e, pcdn_conn conn, uint32_t ring_off, uint32_t len, void* dst);
+/* Pinned host memory holding the frames of a batch: a reference record's raw bytes are at
+ * *host_base + its offset.  Valid until pcdn_release_batch of that batch; PCDN_ENOENT for an unknown or
+ * released batch, and for a device-resident batch (pcdn_submit_device) of an engine without
+ * PCDN_FLAG_SHARED_PAYLOAD, whose frames never reach the host.  Sharded engines and multi-process
+ * groups return this process's own staged copy (identical everywhere by the SPMD contract).       */
+int pcdn_batch_payload(pcdn_engine* e, uint64_t batch_id, const uint8_t** host_base);
 /* PCDN_FLAG_OUTPUT_POOL: run a refused batch (status PCDN_EAGAIN) again after older batches have been
  * released.  Only the oldest unreleased batch can be retried; its result is polled again afterwards.
  * The batch is routed against the tables as they were when it was launched, on every shard, like any
@@ -472,7 +499,10 @@ int pcdn_poll_shard(pcdn_engine* e, uint64_t batch_id, uint32_t local_shard, pcd
  * descriptor attached to its connection with writev — u32 BE length + raw bytes per record, padding
  * skipped, per-connection order kept — on a small thread pool; a failed write detaches the
  * connection and reports it (pcdn_egress_failed), the analogue of the reference removing a peer
- * whose send failed (cdn-broker/src/tasks/user/sender.rs:24-30).                                    */
+ * whose send failed (cdn-broker/src/tasks/user/sender.rs:24-30).
+ * PCDN_FLAG_SHARED_PAYLOAD: the chunks carry the reference records as stored; the fd sink sends each
+ * as two iovecs (the 4 length bytes of the record, the L payload bytes from pcdn_batch_payload), and a
+ * callback sink resolves them the same way through pcdn_batch_payload of the batch it drains.       */
 typedef struct pcdn_egress pcdn_egress;
 typedef struct pcdn_egress_config {
   uint32_t struct_size; /* = sizeof(pcdn_egress_config)                                              */
@@ -524,7 +554,8 @@ int pcdn_set_timing(pcdn_engine* e, int on);
 /* device pointer + geometry of the rings (zero-copy verification / GPUDirect hand-off) */
 int pcdn_ring_info(pcdn_engine* e, void** dev_base, uint64_t* ring_bytes, uint32_t* max_conns);
 /* PCDN_FLAG_HOST_RINGS: host address of the rings (valid for the life of the engine); NULL and
- * PCDN_ENOENT when the rings live in device memory. */
+ * PCDN_ENOENT when the rings live in device memory.  The rings hold records (with
+ * PCDN_FLAG_SHARED_PAYLOAD: reference records, see above). */
 int pcdn_host_rings(pcdn_engine* e, const void** host_base);
 /* number of connected users (Connections::num_users mod.rs:127) and brokers */
 int pcdn_num_users(pcdn_engine* e, uint32_t* users, uint32_t* brokers);

@@ -38,6 +38,8 @@ FLAG_HOST_RINGS = 4     # rings in mapped pinned host memory: spans are readable
 FLAG_OUTPUT_POOL = 16   # one shared output pool per GPU instead of a ring per connection (spans: 32-byte units relative to pool_base)
 FLAG_SPAN_RUNS = 8      # run-length span table (BatchResult.runs): consecutive connections with identical spans
 FLAG_STAGED_SPANS = 2   # force the large-engine span path (table in HBM + D2H) on a small engine
+FLAG_SHARED_PAYLOAD = 32  # every delivery is one 32-byte reference record; the payload exists once per batch (batch_payload)
+REF_MARK = 0xFFFFFFFF     # first 4 bytes of a reference record
 BATCH_READY = 1         # DeviceBatch.hints: the arrays are already complete in device memory
 INGEST_NCCL, INGEST_HOST = 0, 1   # sharded engines: NCCL broadcast over NVLink | every shard copies from host
 RECORD_ALIGN = 32
@@ -224,6 +226,7 @@ ABI = {
     "pcdn_next_batch": (_ci, [_vp, C.POINTER(_u64)]),
     "pcdn_poll": (_ci, [_vp, _u64, C.POINTER(BatchResult), _ci]),
     "pcdn_read": (_ci, [_vp, _u32, _u32, _u32, _vp]),
+    "pcdn_batch_payload": (_ci, [_vp, _u64, C.POINTER(_vp)]),
     "pcdn_release_batch": (_ci, [_vp, _u64]),
     "pcdn_retry_batch": (_ci, [_vp, _u64]),
     "pcdn_nccl_unique_id": (_ci, [_vp]),
@@ -546,6 +549,13 @@ class Engine:
         self._chk(self.L.pcdn_read(self.h, conn, ring_off, length, C.cast(buf, C.c_void_p)))
         return buf.raw[:length]
 
+    def batch_payload(self, batch_id: int) -> int:
+        """host address of the batch's frames (pinned, valid until release): a reference record's raw
+        bytes are at this address + the record's offset"""
+        p = C.c_void_p()
+        self._chk(self.L.pcdn_batch_payload(self.h, batch_id, C.byref(p)))
+        return p.value or 0
+
     def release_batch(self, batch_id: int) -> None:
         self._chk(self.L.pcdn_release_batch(self.h, batch_id))
 
@@ -567,7 +577,8 @@ class Engine:
 
     def collect_frames(self, res: BatchResult) -> Dict[int, List[bytes]]:
         """What the per-connection writer tasks would put on the wire for this batch: walk every
-        span record by record (BE length prefix, 32-byte record stride) and return the raw frames
+        span record by record (BE length prefix, 32-byte record stride; a reference record of a
+        FLAG_SHARED_PAYLOAD engine is resolved through batch_payload) and return the raw frames
         per connection in ring order.  A wrapped connection has two spans: the one that does not
         start at offset 0 comes first."""
         per: Dict[int, List[Tuple[int, int, int]]] = {}
@@ -575,6 +586,8 @@ class Engine:
         stride, rbytes = sh[0].shard_stride, sh[0].ring_bytes
         hosts = {d.global_index: d.rings_host for d in sh if d.rings_host}
         pool = bool(self.cfg.flags & FLAG_OUTPUT_POOL)   # offsets: 32-byte units relative to res.pool_base
+        # shared-payload engines: reference records point into the batch's payload
+        payload = self.batch_payload(res.batch_id) if self.cfg.flags & FLAG_SHARED_PAYLOAD else 0
         for conn, off, ln, nrec in self.spans(res):
             per.setdefault(conn, []).append((off, ln, nrec))
         out: Dict[int, List[bytes]] = {}
@@ -593,6 +606,12 @@ class Engine:
                 p = 0
                 for _ in range(nrec):
                     L = int.from_bytes(data[p:p + 4], "big")
+                    if payload and L == REF_MARK:
+                        L = int.from_bytes(data[p + 4:p + 8], "big")
+                        assert int.from_bytes(data[p + 16:p + 24], "little") == res.batch_id, (conn, p)
+                        frames.append(C.string_at(payload + int.from_bytes(data[p + 8:p + 16], "little"), L))
+                        p += RECORD_ALIGN
+                        continue
                     frames.append(data[p + 4:p + 4 + L])
                     p += (4 + L + RECORD_ALIGN - 1) // RECORD_ALIGN * RECORD_ALIGN
                 assert p == ln, (conn, off, ln, nrec, p)

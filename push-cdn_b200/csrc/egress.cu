@@ -11,7 +11,9 @@
 // c-1), and the sink gets {host bytes, spans, offset of every span}.  Engines with PCDN_FLAG_HOST_RINGS
 // skip all of that: the sink sees the rings in place.  The built-in sink writes every span to the
 // file descriptor attached to its connection with writev (length prefix + raw bytes per record, the
-// padding between records skipped), on a small thread pool, keeping per-connection order.
+// padding between records skipped), on a small thread pool, keeping per-connection order.  On a
+// PCDN_FLAG_SHARED_PAYLOAD engine a reference record becomes two iovecs: its 4 length bytes and the L
+// bytes of the batch's payload (pcdn_batch_payload) it points to.
 #include <errno.h>
 #include <poll.h>
 #include <sys/socket.h>
@@ -147,6 +149,10 @@ struct pcdn_egress {
   std::vector<pcdn_conn> failed, failed_out;
   pcdn_egress_stats last{};
   std::atomic<uint64_t> fd_bytes{0}, fd_writes{0}, unattached{0}, records{0};
+  // PCDN_FLAG_SHARED_PAYLOAD: the batch being drained and its payload base (reference records point into it)
+  const uint8_t* payload = nullptr;
+  uint64_t batch_id = 0;
+  std::atomic<bool> bad_ref{false};
 };
 
 namespace {
@@ -354,14 +360,26 @@ int fd_sink(void* user, const pcdn_egress_chunk* ch) {
       const int fd = s.conn < g->fds.size() ? g->fds[s.conn] : -1;
       if (fd < 0) { una += fd == -1; continue; }
       // walk the records exactly like the writer task walks its queue: u32 BE length, then the bytes
+      // (a reference record: its 4 length bytes, then the L bytes of the shared payload)
       iov.clear();
       const uint8_t* q = ch->data + ch->data_off[i];
+      bool ok = true;
       for (uint32_t r = 0; r < s.n_records; r++) {
+        if (g->payload && be32(q) == PCDN_REF_MARK) {
+          uint64_t off, bid;
+          std::memcpy(&off, q + 8, 8); std::memcpy(&bid, q + 16, 8);
+          if (bid != g->batch_id) { ok = false; break; }
+          iov.push_back({(void*)(q + 4), 4});
+          iov.push_back({(void*)(g->payload + off), be32(q + 4)});
+          q += PCDN_RECORD_ALIGN;
+          continue;
+        }
         const uint32_t F = 4 + be32(q);
         if (!iov.empty() && (const uint8_t*)iov.back().iov_base + iov.back().iov_len == q) iov.back().iov_len += F;
         else iov.push_back({(void*)q, F});
         q += (F + PCDN_RECORD_ALIGN - 1) / PCDN_RECORD_ALIGN * PCDN_RECORD_ALIGN;
       }
+      if (!ok) { g->bad_ref = true; continue; }   // a record of another batch: nothing of this span is written
       nrec += s.n_records;
       if (!write_all(fd, iov.data(), (int)iov.size(), &nb, &nw)) {
         // Err ⇒ the reference's sender removes the peer (tasks/user/sender.rs:24-30): report it, stop writing to it
@@ -372,7 +390,7 @@ int fd_sink(void* user, const pcdn_egress_chunk* ch) {
     }
     g->fd_bytes += nb; g->fd_writes += nw; g->records += nrec; g->unattached += una;
   });
-  return 0;
+  return g->bad_ref ? 1 : 0;
 }
 
 int drain_locked(pcdn_egress* g, uint64_t batch_id, pcdn_egress_sink sink, void* user, pcdn_egress_stats* out) {
@@ -382,6 +400,8 @@ int drain_locked(pcdn_egress* g, uint64_t batch_id, pcdn_egress_sink sink, void*
   const auto t0 = std::chrono::steady_clock::now();
   const uint32_t nl = (uint32_t)e->shards.size();
   int rc = 0;
+  g->payload = nullptr; g->batch_id = batch_id; g->bad_ref = false;
+  if ((e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) && (rc = pcdn_batch_payload(e, batch_id, &g->payload))) return rc;
   if (nl == 1) {
     rc = drain_shard(g, batch_id, 0, sink, user, &st);
   } else {

@@ -213,6 +213,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
     CUDA_TRY(cudaMemsetAsync(s.w.lb_state, 0, ((size_t)sh.dev.N / 256 + 1) * 8, st));
   }
   s.w.pool_unblock = retry ? 1u : 0u;
+  s.w.batch_id = retry ? e->slots[si].batch_id : e->next_batch_id;   // (launch_pipeline hands out next_batch_id)
   // latency path of the smallest geometry: match + plan + offsets in one cluster launch that also
   // zeroes / publishes the counters (kernels.cu: k_ctrl_small)
   // (one cluster of 8 CTAs: worth it while the whole match is a few passes — a 128-message batch on a
@@ -706,7 +707,10 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
   d.N = Ns; d.W = Ws; d.T = g.T; d.nblk = Ws / kBlockWords;
   d.bucket_mask = g.bucket_mask; d.key_stride = g.key_stride; d.seed = g.seed;
   d.ring_bytes = c.ring_bytes_per_conn; d.ring_units = (uint32_t)(c.ring_bytes_per_conn / kUnit);
-  d.cm_enable = (c.pack_variant & 2) ? 0 : 1;
+  d.shared_payload = (c.flags & PCDN_FLAG_SHARED_PAYLOAD) ? 1u : 0u;
+  // (shared payload: every delivery is one 32-byte record with an explicit {conn, off} entry; the
+  //  connection-major class stages frame copies, so it is off)
+  d.cm_enable = ((c.pack_variant & 2) || d.shared_payload) ? 0 : 1;
   d.fat_tile_bytes = (128u << 10) << ((c.pack_variant >> 4) & 15u);  // A/B: bits 4-7 double the tile
   d.fat_grab = 1u << ((c.pack_variant >> 16) & 7u);                   // A/B: bits 16-18 = log2 tiles per cursor update
   d.n_valid_topics = c.n_valid_topics;
@@ -1487,6 +1491,9 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
       b->n_bcast > b->n_msgs)
     return fail(PCDN_EINVAL, "device batch exceeds configured capacities");
   const uint32_t n = b->n_msgs, nb = b->n_bcast;
+  const bool shared = (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) != 0;
+  if (shared && b->arena_bytes > e->arena_cap)
+    return fail(PCDN_ENOSPC, "device batch frames exceed the pinned payload staging (max_batch_bytes)");
   // sharded engines: the frames at the start of a receiving shard's arena, the descriptor block behind them
   const DescLayout L(n, nb, b->n_topics_total);
   const size_t doff = align_up(b->arena_bytes, 256);
@@ -1526,6 +1533,17 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
     else              // where the caller put it
       ss.in = BatchIn{n, nb, (const uint8_t*)b->arena, b->kind, b->flags, b->slot_off16, b->raw_len, b->aux_off, b->aux_len,
                       b->topics, b->bcast_index};
+  }
+  if (shared) {
+    // the payload of the reference records: ONE D2H copy of the frames, from where the first local shard
+    // reads them, on that shard's main stream ahead of the batch's kernels (so its ev_done covers it)
+    Shard& sh = e->shards[0];
+    ShardSlot& ss = sh.slots[si];
+    DeviceGuard dg(sh.device);
+    cudaError_t ce = e->sharded ? cudaStreamWaitEvent(sh.stream, ss.ev_ingest, 0) : cudaSuccess;
+    if (ce == cudaSuccess && b->arena_bytes)
+      ce = cudaMemcpyAsync(s.h_arena, ss.in.arena, b->arena_bytes, cudaMemcpyDeviceToHost, sh.stream);
+    if (ce != cudaSuccess) { abandon_open(e); return fail(PCDN_ECUDA, std::string("payload staging copy: ") + cudaGetErrorString(ce)); }
   }
   s.device_input = true;
   s.n_msgs = n;
@@ -1739,6 +1757,23 @@ int pcdn_read(pcdn_engine* e, pcdn_conn conn, uint32_t ring_off, uint32_t len, v
   GUARD_END
 }
 
+int pcdn_batch_payload(pcdn_engine* e, uint64_t batch_id, const uint8_t** host_base) {
+  GUARD_BEGIN
+  LOCK;
+  if (host_base) *host_base = nullptr;
+  if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine");
+  const int si = find_slot_index(e, batch_id);
+  if (si < 0) return fail(PCDN_ENOENT, "unknown or released batch id");
+  const Slot& s = e->slots[si];
+  // host-staged batches keep their frames in the slot's pinned staging until release; device-resident
+  // ones have them copied there only by shared-payload engines
+  if (s.device_input && !(e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD))
+    return fail(PCDN_ENOENT, "the frames of a device-resident batch are staged on the host only with PCDN_FLAG_SHARED_PAYLOAD");
+  if (host_base) *host_base = s.h_arena;
+  return 0;
+  GUARD_END
+}
+
 int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id) {
   GUARD_BEGIN
   LOCK;
@@ -1779,8 +1814,11 @@ int pcdn_release_batch(pcdn_engine* e, uint64_t batch_id) {
     ShardSlot& ss = sh.slots[si];
     // A slot released without having been polled may still have its host→device staging copy queued:
     // its pinned staging buffers must not be refilled before that copy ran (device-input batches have
-    // no host staging and stay fully asynchronous — the pipelined submit_device/release loop).
-    if (!ss.polled && !s.device_input) CUDA_TRY(cudaEventSynchronize(e->sharded ? ss.ev_ingest : ss.ev_done));
+    // no host staging and stay fully asynchronous — the pipelined submit_device/release loop — unless
+    // their frames are being copied into the staging as the shared payload: ev_done comes after that copy).
+    const bool payload_copy = s.device_input && (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD);
+    if (!ss.polled && (!s.device_input || payload_copy))
+      CUDA_TRY(cudaEventSynchronize((e->sharded && !payload_copy) ? ss.ev_ingest : ss.ev_done));
     if (e->timeline && ss.timed && !e->timeline_async) {   // diagnostic: where this batch's stages ran on the shard's clock (blocks until the pack is done)
       CUDA_TRY(cudaEventSynchronize(ss.ev_done));
       float t[6];

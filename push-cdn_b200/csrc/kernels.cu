@@ -461,6 +461,11 @@ void launch_match(const DevState& s, const Work& w, const BatchIn& b, cudaStream
 // =============================================================================== K1p plan
 __device__ __forceinline__ uint32_t frame_vec_bytes(uint32_t raw_len) { return (4u + raw_len + 15u) & ~15u; }
 __device__ __forceinline__ uint32_t frame_units(uint32_t raw_len) { return (4u + raw_len + kUnit - 1u) / kUnit; }
+// units one delivery takes in a ring / the output pool: the framed copy, or (PCDN_FLAG_SHARED_PAYLOAD)
+// one 32-byte reference record.  Every placement site (k_offsets, its direct path, k_ctrl_small) uses it.
+__device__ __forceinline__ uint32_t rec_units(const DevState& s, uint32_t raw_len) {
+  return s.shared_payload ? 1u : frame_units(raw_len);
+}
 // recipients per message-major tile: about 2 MB of stores per tile whatever the frame size, so a
 // batch of large frames still splits into enough tiles to balance ~450 persistent CTAs
 __device__ __forceinline__ uint32_t tile_recipients(uint32_t frame_bytes, uint32_t tile_bytes) {
@@ -695,7 +700,7 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
   // direct hit: message m owns entry m of the direct list
   auto emit_direct = [&](uint32_t m) {
     const uint32_t len = b.raw_len[m];
-    const uint32_t off = alloc_record(k, frame_units(len), R, len);
+    const uint32_t off = alloc_record(k, rec_units(s, len), R, len);
     w.edir[m] = make_uint2(c, off);
   };
 
@@ -731,7 +736,7 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
       if (HAS_DIRECT) while (dp < de && dmsg[dp] < mb) { emit_direct(dmsg[dp]); dp++; }  // keep batch order (R9)
       if ((word >> lane) & 1u) {
         const uint32_t rank = p + __popc(word & lt), len = m_len[i];
-        const uint32_t off = alloc_record(k, frame_units(len), R, len);
+        const uint32_t off = alloc_record(k, rec_units(s, len), R, len);
         const uint32_t cl = m_cls[i];
         if (cl == CLS_CM) w.ecm[m_eb[i] + rank] = off;
         else if (cl == CLS_FAT) w.efat[m_eb[i] + rank] = make_uint2(c, off);
@@ -1378,7 +1383,55 @@ __global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, W
   pack_direct_phase(s, b, w);
 }
 
+// =============================================================================== K2r pack (reference records)
+// PCDN_FLAG_SHARED_PAYLOAD: every delivery is ONE 32-byte reference record (pcdn_fanout.h) instead of a
+// framed copy: marker, BE length, offset of the raw bytes in the batch's frame arena, batch id, zero.
+// One sector, two 16-byte streaming stores, no partial-sector write.  The record depends on the message
+// and the batch only, so a retried batch writes identical records wherever the pool places them.
+__device__ __forceinline__ void st_ref_record(uint8_t* dst, uint32_t raw_len, uint32_t slot_off16, unsigned long long batch_id) {
+  const unsigned long long off = (unsigned long long)slot_off16 * 16u + 4u;
+  st_stream16(dst, make_uint4(0xFFFFFFFFu, bswap32(raw_len), (uint32_t)off, (uint32_t)(off >> 32)));
+  st_stream16(dst + 16, make_uint4((uint32_t)batch_id, (uint32_t)(batch_id >> 32), 0u, 0u));
+}
+// Thread per delivery over the three scatter lists back to back: message-major (efat: the owning message
+// is found by a binary search of eb_fat), thin (ethin carries everything) and direct (edir, entry m =
+// message m).  Entries of one message are in connection order, so a warp's 32 stores go to 32
+// consecutive connections; a connection's records of successive messages are adjacent in its ring.
+__global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w, int do_direct) {
+  if (w.stats->status) return;
+  const uint32_t nfat = w.stats->n_fat_entries, nthin = w.stats->n_thin_entries;
+  const uint64_t nft = (uint64_t)nfat + nthin, total = nft + (do_direct ? b.n_msgs : 0u);
+  const uint32_t pool_base = w.stats->pool_base;
+  const unsigned long long bid = w.batch_id;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    uint32_t conn, off, m = 0, slot = 0, len = 0;
+    bool thin = false;
+    if (i < nfat) {
+      const uint32_t e = (uint32_t)i;
+      uint32_t lo = 0, hi = b.n_msgs;  // largest m with eb_fat[m] <= e: the message that owns entry e
+      while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (w.eb_fat[mid] <= e) lo = mid; else hi = mid; }
+      const uint2 ent = w.efat[e];
+      conn = ent.x; off = ent.y; m = lo;
+    } else if (i < nft) {
+      const uint4 ent = w.ethin[i - nfat];
+      conn = ent.x; off = ent.y; slot = ent.z; len = ent.w; thin = true;
+    } else {
+      m = (uint32_t)(i - nft);
+      const uint2 ent = w.edir[m];
+      conn = ent.x; off = ent.y;
+    }
+    if (off == kOffInvalid) continue;   // ring overflow, or a direct message this shard does not deliver
+    if (!thin) { slot = b.slot_off16[m]; len = b.raw_len[m]; }
+    st_ref_record(conn_out(s, w, conn, pool_base) + (size_t)off * kUnit, len, slot, bid);
+  }
+}
+
 void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t variant, int n_sms, cudaStream_t st) {
+  if (s.shared_payload) {   // (the pack_variant geometry bits describe k_pack: they do not apply here)
+    if (b.n_bcast || n_direct) PCDN_COUNT_LAUNCH, k_pack_ref<<<(uint32_t)n_sms * 8, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0);
+    return;
+  }
   const bool direct_separate = n_direct >= kThinSeparateMin;
   // Default (variant 0): TMA bulk stores; CTAs per SM come from the engine (launch_shard_pipeline), else 3.
   // A/B switches for profiling: bit 2 = st.global.cs.v4 stores instead of bulk stores; bit 1 = no

@@ -17,6 +17,8 @@
 //                       records), message-major (16 KiB chunks staged once per CTA, replicated to
 //                       ~128 KB worth of recipients per tile), thin (warp per delivery; its own
 //                       full-occupancy launch k_pack_thin for batches of >= 2048 direct messages)
+//   K2r k_pack_ref      (PCDN_FLAG_SHARED_PAYLOAD) replaces K2: thread per delivery over the three scatter
+//                       lists, one 32-byte reference record each (the payload stays once per batch)
 //   K1s k_ctrl_small    latency path (N <= 65536 connection slots, <= 256 messages): K3 + sort + K1a +
 //                       K1p + K1b in ONE cluster launch, counters/spans published to mapped host memory
 //   K4  k_apply_*       scatter of changed table words/slots (subscribe, add/remove, direct map)
@@ -91,6 +93,7 @@ struct DevState {
   uint32_t conn_base;
   uint32_t span_runs;    // PCDN_FLAG_SPAN_RUNS: the span table is run-length encoded (SpanRun entries)
   uint32_t count_drops;  // 1 on exactly one shard of the broker (global shard 0): it counts the unroutable directs
+  uint32_t shared_payload;  // PCDN_FLAG_SHARED_PAYLOAD: one 32-byte reference record per delivery (k_pack_ref), no cm class
   uint64_t ring_bytes;
   uint64_t seed;
 };
@@ -188,6 +191,7 @@ struct Work {
   unsigned long long* lb_state;  // [N / 256 + 1] look-back words (fused small-engine kernel)
   uint32_t* lb_tot;      // [N / 256 + 1] units per k_offsets CTA (regular kernel; finished by k_pool_finish)
   uint32_t pool_unblock; // this launch is the retry of the oldest refused batch: clear PoolState::blocked
+  unsigned long long batch_id;  // the batch this launch packs (k_pack_ref writes it into every reference record)
   // outputs
   uint32_t* batch_units; // [N] units consumed by this batch per connection (for release)
   Span* spans;           // [2*N] spans, or (span_runs) [2*N] SpanRun entries in the same buffer (sized for the larger)
