@@ -457,7 +457,7 @@ int before_state_change(pcdn_engine* e) {
 struct InMsg {
   uint8_t kind, flags;
   bool prune;                        // broadcast: apply Topic::prune to the wire topic list
-  uint32_t raw_len, key_len;         // key_len: direct message's recipient length (0 = no recipient)
+  uint32_t raw_len, key_len;         // key_len: direct message's recipient length (routed_key_len)
   uint32_t n_listed, n_topics;       // broadcast: entries of the topic list below, entries it adds to the batch
   const uint8_t* raw;
   const uint8_t* key;                // direct: the recipient
@@ -508,8 +508,10 @@ bool pool_admits(const pcdn_engine* e, uint64_t bytes) {
 }
 
 // A recipient longer than any key in the table cannot match (bytewise identity, R8): the message is
-// dropped, but batch order bookkeeping still wants it, so it is routed as "no recipient".
-uint32_t routed_key_len(const pcdn_engine* e, uint32_t len) { return len > e->cfg.max_key_len ? 0 : len; }
+// dropped, but batch order bookkeeping still wants it.  It is staged as its first max_key_len + 1
+// bytes, a length no table entry has, so the lookup finds no candidate and counts the drop.  (Length 0
+// would not do: that is the key of a user whose key is empty.)
+uint32_t routed_key_len(const pcdn_engine* e, uint32_t len) { return len > e->cfg.max_key_len ? e->cfg.max_key_len + 1 : len; }
 
 // a message of the C ABI's handle / submit calls
 InMsg api_msg(const pcdn_engine* e, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
@@ -1451,7 +1453,7 @@ static int validate_explicit_batch(pcdn_engine* e, const pcdn_msg* msgs, uint32_
       return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": null pointer with non-zero length");
     if (const char* why = msg_invalid(e, m.raw_len)) return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": " + why);
     const bool direct = m.kind == PCDN_KIND_DIRECT;
-    const MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(std::min<uint32_t>(m.recipient_len, c.max_key_len), 16) : 0u,
+    const MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(std::min<uint32_t>(m.recipient_len, c.max_key_len + 1), 16) : 0u,
                          direct ? 0u : m.n_topics};
     if (!full) full = batch_limit(e, fill, shape);
     fill.add(shape);

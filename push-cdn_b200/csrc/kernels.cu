@@ -167,7 +167,10 @@ __global__ void __launch_bounds__(256) k_parse(DevState s, BatchIn b, Work w) {
     }
   } else {  // direct: recipient key in place (word aligned in a valid message)
     aoff = slot_b + 4 + pf.f0_off; alen = pf.f0_len;
-    if (alen > s.max_key_len || (aoff & 3)) kind = 0;  // longer than any registered key: no route
+    if (aoff & 3) kind = 0;
+    // longer than any registered key: its first max_key_len + 1 bytes match no entry, so the lookup
+    // drops it and counts it, as the host staging does (engine.cu routed_key_len)
+    else if (alen > s.max_key_len) alen = s.max_key_len + 1;
   }
   const_cast<uint8_t*>(b.kind)[m] = kind;
   const_cast<uint8_t*>(b.flags)[m] = fl;

@@ -17,12 +17,12 @@ ENOSPC, EAGAIN = -5, -11
 
 def _staged(msgs, max_key_len):
     """bytes an explicit batch may stage: 16-byte frame slots plus, for direct messages, the key
-    staged beside the frame (the worst case)"""
+    staged beside the frame (the worst case; a longer recipient as its first max_key_len + 1 bytes)"""
     n = 0
     for m in msgs:
         n += (4 + len(m[2]) + 15) // 16 * 16
         if m[0] == "d":
-            n += (min(len(m[1]), max_key_len) + 15) // 16 * 16
+            n += (min(len(m[1]), max_key_len + 1) + 15) // 16 * 16
     return n
 
 
