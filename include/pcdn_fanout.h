@@ -97,7 +97,9 @@ typedef struct pcdn_config {
   uint64_t hash_seed;           /* keys the direct-map hash (0 = default)                       */
   void* stream;                 /* optional cudaStream_t to run on (e.g. torch's); NULL = own   */
   const char* identity;         /* this broker's BrokerIdentifier string "public/private"       */
-  uint32_t pack_variant;        /* 0 = default; see DESIGN.md (kernel selection for profiling)  */
+  uint32_t pack_variant;        /* pack launch geometry, 0 = engine default.  Bits 8-11 (k_pack) and
+                                 * 12-15 (k_pack_direct), when non-zero, override the CTAs per SM;
+                                 * any other bit set is PCDN_EINVAL.  Output does not depend on it. */
   uint32_t flags;               /* PCDN_FLAG_*                                                  */
   /* ---- connection shards over several GPUs (SURVEY 8e) ---------------------------------------
    * n_devices > 1 (or world_shards > 1): `max_conns`, `ring_bytes_per_conn` and the batch capacities
@@ -182,8 +184,8 @@ enum {
    * reference's fan-out clones a refcounted `Bytes`, it never copies per recipient).  Spans, runs,
    * n_records, pool_base, wrap, release and retry keep their meaning; bytes_out still counts the 4 + L
    * wire bytes of each delivery.  Records have no size limit in this mode (one unit each), so messages
-   * far larger than a ring are delivered.  The pack geometry bits of pcdn_config.pack_variant do not
-   * apply (the pack kernel is k_pack_ref).  Record layout (all fields fixed, so bytes compare exactly):
+   * far larger than a ring are delivered.  The CTA counts of pcdn_config.pack_variant do not apply
+   * (the pack kernel is k_pack_ref).  Record layout (all fields fixed, so bytes compare exactly):
    *   bytes  0..3   PCDN_REF_MARK (no framed record starts with it: L <= 0x1FFFFFFF)
    *   bytes  4..7   u32 big-endian L: the 4 wire bytes of the length prefix
    *   bytes  8..15  u64 little-endian offset of the raw bytes from the batch's payload base

@@ -164,9 +164,8 @@ static constexpr uint32_t kTimelineBatches = 64;
 int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_direct, bool devparse, bool wait_ingest, bool retry = false) {
   DeviceGuard dg(sh.device);
   ShardSlot& s = sh.slots[si];
-  // Default: the pack runs on the main stream.  A/B switch (pack_variant bit 3): run it on the
-  // high-priority pack stream so the next batch's control kernels overlap it — slower for a long
-  // bulk-store pack, so it stays opt-in.
+  // Default: the pack runs on the main stream.  On the high-priority pack stream the next batch's control
+  // kernels overlap it, which is slower for a long bulk-store pack; so only the batches below take it.
   const bool dp = sh.direct_publish;
   // Batches of nothing but many direct messages DO take the pack stream: their control kernels are
   // latency-bound (three dependent random reads per message), their pack is a separate bandwidth-bound
@@ -188,10 +187,10 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
       break;
     }
   }
-  const bool fat_overlap = s.in.n_bcast > 0 && sh.fat_only && !(e->cfg.pack_variant & 32);   // (bit 5: A/B switch, never overlap broadcast batches)
+  const bool fat_overlap = s.in.n_bcast > 0 && sh.fat_only;
   sh.prev_slot[1] = sh.prev_slot[0];
   sh.prev_slot[0] = (int)si;
-  cudaStream_t st = sh.stream, ps = (!dp && ((e->cfg.pack_variant & 8) || direct_only || fat_overlap)) ? sh.pack_stream : sh.stream, cs = sh.copy_stream;
+  cudaStream_t st = sh.stream, ps = (!dp && (direct_only || fat_overlap)) ? sh.pack_stream : sh.stream, cs = sh.copy_stream;
   const bool has_direct = n_direct > 0;
   if (wait_ingest) CUDA_TRY(cudaStreamWaitEvent(st, s.ev_ingest, 0));
   s.timed = e->timing && !e->timeline_async;
@@ -710,11 +709,6 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
   d.bucket_mask = g.bucket_mask; d.key_stride = g.key_stride; d.seed = g.seed;
   d.ring_bytes = c.ring_bytes_per_conn; d.ring_units = (uint32_t)(c.ring_bytes_per_conn / kUnit);
   d.shared_payload = (c.flags & PCDN_FLAG_SHARED_PAYLOAD) ? 1u : 0u;
-  // (shared payload: every delivery is one 32-byte record with an explicit {conn, off} entry; the
-  //  connection-major class stages frame copies, so it is off)
-  d.cm_enable = ((c.pack_variant & 2) || d.shared_payload) ? 0 : 1;
-  d.fat_tile_bytes = (128u << 10) << ((c.pack_variant >> 4) & 15u);  // A/B: bits 4-7 double the tile
-  d.fat_grab = 1u << ((c.pack_variant >> 16) & 7u);                   // A/B: bits 16-18 = log2 tiles per cursor update
   d.n_valid_topics = c.n_valid_topics;
   d.max_key_len = c.max_key_len;
   d.conn_base = sh.gindex * Ns;
@@ -926,6 +920,8 @@ int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
   if (cfg->ring_bytes_per_conn % PCDN_RECORD_ALIGN || cfg->ring_bytes_per_conn == 0 || cfg->ring_bytes_per_conn > (1ull << 31))
     return fail(PCDN_EINVAL, "ring_bytes_per_conn must be a multiple of 32, at most 2 GiB");
   if (cfg->max_key_len > 4096) return fail(PCDN_EINVAL, "max_key_len > 4096");
+  if (cfg->pack_variant & ~0xFF00u)
+    return fail(PCDN_EINVAL, "pack_variant: only the CTA-count fields remain (bits 8-11: k_pack, bits 12-15: k_pack_direct CTAs per SM)");
   // ---- connection shards
   const uint32_t n_local = cfg->n_devices ? cfg->n_devices : 1;
   const uint32_t world = cfg->world_shards ? cfg->world_shards : n_local;

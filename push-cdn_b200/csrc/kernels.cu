@@ -469,11 +469,11 @@ __device__ __forceinline__ uint32_t frame_units(uint32_t raw_len) { return (4u +
 __device__ __forceinline__ uint32_t rec_units(const DevState& s, uint32_t raw_len) {
   return s.shared_payload ? 1u : frame_units(raw_len);
 }
-// recipients per message-major tile: about 2 MB of stores per tile whatever the frame size, so a
+// recipients per message-major tile: about kFatTileBytes of stores per tile whatever the frame size, so a
 // batch of large frames still splits into enough tiles to balance ~450 persistent CTAs
-__device__ __forceinline__ uint32_t tile_recipients(uint32_t frame_bytes, uint32_t tile_bytes) {
+__device__ __forceinline__ uint32_t tile_recipients(uint32_t frame_bytes) {
   const uint32_t chunk = min(frame_bytes, kChunkBytes);
-  return max(32u, min(kTileRecipients, tile_bytes / chunk));
+  return max(32u, min(kTileRecipients, kFatTileBytes / chunk));
 }
 
 // pack class of a message with d recipients, and its number of message-major tiles
@@ -482,13 +482,15 @@ __device__ __forceinline__ void plan_classify(const DevState& s, const BatchIn& 
   uint32_t cls = CLS_THIN, tiles = 0;
   if (d >= kFatMin) {
     const uint32_t len = b.raw_len[m];
-    const bool dense = s.cm_enable && ((uint64_t)d << kCmDenseShift) >= s.N && b.kind[m] == 4;
+    // (shared payload: every delivery is one 32-byte record with an explicit {conn, off} entry; the
+    //  connection-major class stages frame copies, so it is off)
+    const bool dense = !s.shared_payload && ((uint64_t)d << kCmDenseShift) >= s.N && b.kind[m] == 4;
     if (dense && frame_units(len) * kUnit <= kCmMaxBytes) {
       cls = CLS_CM;
     } else {
       cls = CLS_FAT;
       const uint32_t nch = (frame_vec_bytes(len) + kChunkBytes - 1) / kChunkBytes;
-      const uint32_t tr = tile_recipients(frame_vec_bytes(len), s.fat_tile_bytes);
+      const uint32_t tr = tile_recipients(frame_vec_bytes(len));
       tiles = nch * ((d + tr - 1) / tr);
     }
   }
@@ -1041,34 +1043,29 @@ __device__ __forceinline__ uint8_t* conn_out(const DevState& s, const Work& w, u
 // Persistent CTAs pull tiles (message, frame chunk, group of <=1024 recipients) from a counter.
 // The chunk is staged ONCE per CTA into shared memory with a TMA bulk copy (mbarrier-completed),
 // the 4-byte hole at the front of the slot is overwritten with the big-endian length (the
-// cdn-proto framing, protocols/mod.rs:366-385), then every recipient gets the chunk:
-//   VARIANT 0: lanes keep their 16-byte pieces in registers and issue st.global.cs.v4 per recipient
-//   VARIANT 1: one TMA bulk store (shared → global) per recipient, one lane each
-template <int VARIANT>
+// cdn-proto framing, protocols/mod.rs:366-385), then every recipient gets the chunk with one TMA
+// bulk store (shared → global), one lane per recipient.
 __device__ __forceinline__ void pack_fat_phase(const DevState& s, const BatchIn& b, const Work& w, uint8_t* buf,
                                                uint64_t* barp) {
   uint64_t& bar = *barp;
   __shared__ uint32_t t_info[8];  // tile, m, chunk, r0, r1, nbytes, need_load
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t tid = threadIdx.x;
   const uint32_t ntiles = w.stats->n_fat_tiles;
   if (ntiles == 0) return;
   const uint32_t pool_base = w.stats->pool_base;
   uint32_t phase = 0;
   uint32_t staged_m = 0xFFFFFFFFu, staged_k = 0xFFFFFFFFu;  // meaningful in thread 0 only
 
-  uint32_t grab_next = 0, grab_left = 0;  // thread 0: consecutive tiles taken with one cursor update (s.fat_grab of them)
   for (;;) {
     if (tid == 0) {
-      if (grab_left == 0) { grab_next = atomicAdd(&w.stats->tile_cursor, s.fat_grab); grab_left = s.fat_grab; }
-      const uint32_t t = grab_next++;
-      grab_left--;
+      const uint32_t t = atomicAdd(&w.stats->tile_cursor, 1u);
       t_info[0] = t;
       if (t < ntiles) {
         uint32_t lo = 0, hi = b.n_msgs;  // largest m with tbase[m] <= t
         while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (w.tbase[mid] <= t) lo = mid; else hi = mid; }
         const uint32_t m = lo, ltile = t - w.tbase[m], d = w.D[m];
         const uint32_t fb = frame_vec_bytes(b.raw_len[m]);
-        const uint32_t tr = tile_recipients(fb, s.fat_tile_bytes);
+        const uint32_t tr = tile_recipients(fb);
         const uint32_t ngrp = (d + tr - 1) / tr;
         const uint32_t ch = ltile / ngrp, grp = ltile % ngrp;
         const uint32_t nbytes = min(kChunkBytes, fb - ch * kChunkBytes);
@@ -1083,7 +1080,7 @@ __device__ __forceinline__ void pack_fat_phase(const DevState& s, const BatchIn&
     const uint32_t m = t_info[1], ch = t_info[2], r0 = t_info[3], r1 = t_info[4], nbytes = t_info[5];
     if (t_info[6]) {
       // re-stage: drain the bulk stores that still read the old chunk (only here, not per tile)
-      if (VARIANT == 1) bulk_wait_read0();
+      bulk_wait_read0();
       __syncthreads();
       if (tid == 0) {
         mbar_arrive_expect_tx(&bar, nbytes);
@@ -1094,59 +1091,22 @@ __device__ __forceinline__ void pack_fat_phase(const DevState& s, const BatchIn&
       if (ch == 0) {  // fused framing: BE length prefix
         if (tid == 0) {
           *reinterpret_cast<uint32_t*>(buf) = bswap32(b.raw_len[m]);
-          if (VARIANT == 1) fence_proxy_async_smem();
+          fence_proxy_async_smem();
         }
         __syncthreads();
       }
     }
     const uint2* E = w.efat + w.eb_fat[m];
     const size_t chunk_off = (size_t)ch * kChunkBytes;
-    const uint32_t nvec = nbytes >> 4;
-
-    if (VARIANT == 1) {
-      for (uint32_t r = r0 + tid; r < r1; r += 256) {
-        const uint2 ent = E[r];
-        if (ent.y != kOffInvalid)
-          bulk_s2g(conn_out(s, w, ent.x, pool_base) + (size_t)ent.y * kUnit + chunk_off, buf, nbytes);
-      }
-      bulk_commit();
-    } else if (nvec <= 128) {
-      // frame chunk fits 4 registers per lane: load once, then pure store stream
-      uint4 v0, v1, v2, v3;
-      const uint4* sb = reinterpret_cast<const uint4*>(buf);
-      v0 = lane < nvec ? sb[lane] : make_uint4(0, 0, 0, 0);
-      v1 = lane + 32 < nvec ? sb[lane + 32] : make_uint4(0, 0, 0, 0);
-      v2 = lane + 64 < nvec ? sb[lane + 64] : make_uint4(0, 0, 0, 0);
-      v3 = lane + 96 < nvec ? sb[lane + 96] : make_uint4(0, 0, 0, 0);
-      for (uint32_t r = r0 + warp * 32; r < r1; r += 8 * 32) {
-        const uint2 ent = (r + lane < r1) ? E[r + lane] : make_uint2(0, kOffInvalid);
-        const uint32_t cnt = min(32u, r1 - r);
-        for (uint32_t i = 0; i < cnt; i++) {
-          const uint32_t conn = __shfl_sync(0xffffffffu, ent.x, i), off = __shfl_sync(0xffffffffu, ent.y, i);
-          if (off == kOffInvalid) continue;
-          uint4* dst = reinterpret_cast<uint4*>(conn_out(s, w, conn, pool_base) + (size_t)off * kUnit + chunk_off);
-          if (lane < nvec) st_stream16(dst + lane, v0);
-          if (lane + 32 < nvec) st_stream16(dst + lane + 32, v1);
-          if (lane + 64 < nvec) st_stream16(dst + lane + 64, v2);
-          if (lane + 96 < nvec) st_stream16(dst + lane + 96, v3);
-        }
-      }
-    } else {
-      const uint4* sb = reinterpret_cast<const uint4*>(buf);
-      for (uint32_t r = r0 + warp * 32; r < r1; r += 8 * 32) {
-        const uint2 ent = (r + lane < r1) ? E[r + lane] : make_uint2(0, kOffInvalid);
-        const uint32_t cnt = min(32u, r1 - r);
-        for (uint32_t i = 0; i < cnt; i++) {
-          const uint32_t conn = __shfl_sync(0xffffffffu, ent.x, i), off = __shfl_sync(0xffffffffu, ent.y, i);
-          if (off == kOffInvalid) continue;
-          uint4* dst = reinterpret_cast<uint4*>(conn_out(s, w, conn, pool_base) + (size_t)off * kUnit + chunk_off);
-          for (uint32_t v = lane; v < nvec; v += 32) st_stream16(dst + v, sb[v]);
-        }
-      }
+    for (uint32_t r = r0 + tid; r < r1; r += 256) {
+      const uint2 ent = E[r];
+      if (ent.y != kOffInvalid)
+        bulk_s2g(conn_out(s, w, ent.x, pool_base) + (size_t)ent.y * kUnit + chunk_off, buf, nbytes);
     }
+    bulk_commit();
     __syncthreads();  // all reads of t_info done before thread 0 starts the next tile
   }
-  if (VARIANT == 1) bulk_wait_read0();
+  bulk_wait_read0();
 }
 
 // =============================================================================== K2c pack (connection-major)
@@ -1159,9 +1119,7 @@ __device__ __forceinline__ void pack_fat_phase(const DevState& s, const BatchIn&
 // are written as ONE contiguous run — for the all-subscribed case that is the whole batch
 // (8 x 1088 B = 8.7 KB) per connection instead of eight separate 1 KB writes, which is what the
 // HBM row buffers want (scattered 1 KB granules are written well below the copy rate, runs of several KB close to it).
-//   VARIANT 0: the warp copies a connection's run with 16-byte shared loads + st.global.cs.v4
-//   VARIANT 1: every lane issues one TMA bulk store (shared → global) per run of ITS connection
-template <int VARIANT>
+// Every lane issues one TMA bulk store (shared → global) per run of ITS connection.
 __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& b, const Work& w, uint8_t* buf,
                                               uint64_t* barp) {
   uint64_t& bar = *barp;
@@ -1197,7 +1155,7 @@ __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& 
       // New group: shared memory is re-staged.  Bulk stores issued for earlier tiles only have to
       // be drained HERE (they read the old frames) — not after every tile, so the TMA store
       // queue never runs dry while the next tile's offsets are being fetched.
-      if (VARIANT == 1) bulk_wait_read0();
+      bulk_wait_read0();
       __syncthreads();
       if (tid == 0) {
         const uint32_t g = t_info[1];
@@ -1218,7 +1176,7 @@ __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& 
       phase ^= 1;
       if (tid < gcount) {  // fused framing: one BE length prefix per staged frame
         *reinterpret_cast<uint32_t*>(buf + g_soff[tid]) = bswap32(b.raw_len[g_m[tid]]);
-        if (VARIANT == 1) fence_proxy_async_smem();
+        fence_proxy_async_smem();
       }
       __syncthreads();
     }
@@ -1241,61 +1199,25 @@ __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& 
           offs[i] = w.ecm[idx];
         }
       }
-      if (VARIANT == 1) {
-        // one lane = one connection: merge adjacent records into runs, one bulk store per run
-        uint8_t* ring = conn_out(s, w, wd * 32 + lane, pool_base);
-        uint32_t run_o = kOffInvalid, run_units = 0, run_s = 0;
+      // one lane = one connection: merge adjacent records into runs, one bulk store per run
+      uint8_t* ring = conn_out(s, w, wd * 32 + lane, pool_base);
+      uint32_t run_o = kOffInvalid, run_units = 0, run_s = 0;
 #pragma unroll
-        for (int i = 0; i < (int)kCmGroup; i++) {
-          const uint32_t o = offs[i];
-          if (o != kOffInvalid && run_o != kOffInvalid && o == run_o + run_units) {
-            run_units += g_units[i];
-          } else {
-            if (run_o != kOffInvalid) bulk_s2g(ring + (size_t)run_o * kUnit, buf + run_s, run_units * kUnit);
-            run_o = o; run_s = g_soff[i]; run_units = (o != kOffInvalid) ? g_units[i] : 0;
-          }
-        }
-        if (run_o != kOffInvalid) bulk_s2g(ring + (size_t)run_o * kUnit, buf + run_s, run_units * kUnit);
-      } else {
-        uint32_t rem = any;
-        while (rem) {
-          const int l = __ffs(rem) - 1;
-          rem &= rem - 1;
-          uint8_t* ring = conn_out(s, w, wd * 32 + l, pool_base);
-          uint32_t run_o = kOffInvalid, run_units = 0, run_s = 0;
-#pragma unroll
-          for (int i = 0; i <= (int)kCmGroup; i++) {
-            const uint32_t o = i < (int)kCmGroup ? __shfl_sync(0xffffffffu, offs[i < (int)kCmGroup ? i : 0], l) : kOffInvalid;
-            if (o != kOffInvalid && run_o != kOffInvalid && o == run_o + run_units) {
-              run_units += g_units[i];
-            } else {
-              if (run_o != kOffInvalid) {  // warp-cooperative copy of one contiguous run
-                const uint4* src = reinterpret_cast<const uint4*>(buf + run_s);
-                uint4* dst = reinterpret_cast<uint4*>(ring + (size_t)run_o * kUnit);
-                const uint32_t nvec = run_units * 2;
-                for (uint32_t v = lane; v < nvec; v += 128) {
-                  const bool p1 = v + 32 < nvec, p2 = v + 64 < nvec, p3 = v + 96 < nvec;
-                  uint4 x0 = src[v], x1, x2, x3;
-                  if (p1) x1 = src[v + 32];
-                  if (p2) x2 = src[v + 64];
-                  if (p3) x3 = src[v + 96];
-                  st_stream16(dst + v, x0);
-                  if (p1) st_stream16(dst + v + 32, x1);
-                  if (p2) st_stream16(dst + v + 64, x2);
-                  if (p3) st_stream16(dst + v + 96, x3);
-                }
-              }
-              run_o = o;
-              if (i < (int)kCmGroup) { run_s = g_soff[i]; run_units = (o != kOffInvalid) ? g_units[i] : 0; }
-            }
-          }
+      for (int i = 0; i < (int)kCmGroup; i++) {
+        const uint32_t o = offs[i];
+        if (o != kOffInvalid && run_o != kOffInvalid && o == run_o + run_units) {
+          run_units += g_units[i];
+        } else {
+          if (run_o != kOffInvalid) bulk_s2g(ring + (size_t)run_o * kUnit, buf + run_s, run_units * kUnit);
+          run_o = o; run_s = g_soff[i]; run_units = (o != kOffInvalid) ? g_units[i] : 0;
         }
       }
+      if (run_o != kOffInvalid) bulk_s2g(ring + (size_t)run_o * kUnit, buf + run_s, run_units * kUnit);
     }
-    if (VARIANT == 1) bulk_commit();
+    bulk_commit();
     __syncthreads();  // all reads of g_* / t_info done before thread 0 starts the next tile
   }
-  if (VARIANT == 1) bulk_wait_read0();  // the next phase reuses buf
+  bulk_wait_read0();  // the next phase reuses buf
 }
 
 // =============================================================================== K2b pack (thin / direct)
@@ -1360,7 +1282,6 @@ __device__ __forceinline__ void pack_direct_phase(const DevState& s, const Batch
 // One launch runs the pack phases back to back in persistent CTAs (each phase pulls its own
 // work from its own cursor, so CTAs drift from phase to phase without a grid barrier; the phases
 // write disjoint records).
-template <int VARIANT>
 __global__ void __launch_bounds__(256) k_pack(DevState s, BatchIn b, Work w, int do_direct) {
   __shared__ __align__(128) uint8_t buf[kCmGroup * kCmMaxBytes];  // 32 KB; the fat phase uses the first 16 KB
   __shared__ __align__(8) uint64_t bars[2];
@@ -1371,9 +1292,9 @@ __global__ void __launch_bounds__(256) k_pack(DevState s, BatchIn b, Work w, int
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  pack_cm_phase<VARIANT>(s, b, w, buf, &bars[0]);
+  pack_cm_phase(s, b, w, buf, &bars[0]);
   __syncthreads();
-  pack_fat_phase<VARIANT>(s, b, w, buf, &bars[1]);
+  pack_fat_phase(s, b, w, buf, &bars[1]);
   pack_thin_phase(s, b, w);
   if (do_direct) pack_direct_phase(s, b, w);
 }
@@ -1430,25 +1351,22 @@ __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w,
   }
 }
 
-void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t variant, int n_sms, cudaStream_t st) {
-  if (s.shared_payload) {   // (the pack_variant geometry bits describe k_pack: they do not apply here)
+// pack_variant (pcdn_config) holds launch geometry only: bits 8-11 = CTAs per SM of k_pack (the engine
+// fills in its default, launch_shard_pipeline; 3 if none), bits 12-15 = CTAs per SM of the separate
+// direct pack (default 8 = full occupancy).  Neither changes what is written, only how the persistent
+// CTAs share the work.
+void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms, cudaStream_t st) {
+  if (s.shared_payload) {   // (the CTA counts of pack_variant describe k_pack and k_pack_direct: they do not apply here)
     if (b.n_bcast || n_direct) PCDN_COUNT_LAUNCH, k_pack_ref<<<(uint32_t)n_sms * 8, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0);
     return;
   }
   const bool direct_separate = n_direct >= kThinSeparateMin;
-  // Default (variant 0): TMA bulk stores; CTAs per SM come from the engine (launch_shard_pipeline), else 3.
-  // A/B switches for profiling: bit 2 = st.global.cs.v4 stores instead of bulk stores; bit 1 = no
-  // connection-major class (DevState::cm_enable, read by k_plan_a); bits 4-7 = log2 multiplier of
-  // the 128 KB message-major tile (DevState::fat_tile_bytes); bits 8+ = CTAs per SM.
-  const uint32_t ctas_per_sm = ((variant >> 8) & 15u) ? ((variant >> 8) & 15u) : 3;
+  const uint32_t ctas_per_sm = ((pack_variant >> 8) & 15u) ? ((pack_variant >> 8) & 15u) : 3;
   const uint32_t grid = (uint32_t)n_sms * ctas_per_sm;
   const int do_direct = (n_direct && !direct_separate) ? 1 : 0;
-  if (b.n_bcast || do_direct) {  // (a batch of nothing but many direct messages has no work for this kernel)
-    if (variant & 4) PCDN_COUNT_LAUNCH, k_pack<0><<<grid, 256, 0, st>>>(s, b, w, do_direct);
-    else PCDN_COUNT_LAUNCH, k_pack<1><<<grid, 256, 0, st>>>(s, b, w, do_direct);
-  }
-  // (A/B: bits 12-15 = CTAs per SM of the separate direct pack, default 8 = full occupancy)
-  const uint32_t dctas = ((variant >> 12) & 15u) ? ((variant >> 12) & 15u) : 8u;
+  if (b.n_bcast || do_direct)  // (a batch of nothing but many direct messages has no work for this kernel)
+    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct);
+  const uint32_t dctas = ((pack_variant >> 12) & 15u) ? ((pack_variant >> 12) & 15u) : 8u;
   if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w);
 }
 

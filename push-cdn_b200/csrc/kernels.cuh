@@ -15,8 +15,9 @@
 //   K2  k_pack          persistent CTAs, three phases: connection-major (groups of <= 8 small frames
 //                       staged by TMA, one TMA bulk store per contiguous run of a connection's
 //                       records), message-major (16 KiB chunks staged once per CTA, replicated to
-//                       ~128 KB worth of recipients per tile), thin (warp per delivery; its own
-//                       full-occupancy launch k_pack_thin for batches of >= 2048 direct messages)
+//                       ~128 KB worth of recipients per tile), thin (warp per delivery), direct (warp
+//                       per message; its own full-occupancy launch k_pack_direct for batches of >= 2048
+//                       direct messages)
 //   K2r k_pack_ref      (PCDN_FLAG_SHARED_PAYLOAD) replaces K2: thread per delivery over the three scatter
 //                       lists, one 32-byte reference record each (the payload stays once per batch)
 //   K1s k_ctrl_small    latency path (N <= 65536 connection slots, <= 256 messages): K3 + sort + K1a +
@@ -36,7 +37,8 @@ constexpr uint32_t kOffInvalid = 0xFFFFFFFFu;
 constexpr uint32_t kConnNone = 0xFFFFFFFFu;
 constexpr uint32_t kFatMin = 32;             // >= this many recipients → staged (fat) path
 constexpr uint32_t kChunkBytes = 16384;      // shared-memory staging chunk of the fat path
-constexpr uint32_t kTileRecipients = 1024;   // recipients per fat tile
+constexpr uint32_t kTileRecipients = 1024;   // most recipients per fat tile
+constexpr uint32_t kFatTileBytes = 131072;   // bytes of stores a fat tile aims at (kernels.cu: tile_recipients)
 constexpr uint32_t kBlockWords = 256;        // bitmap words per match block (8192 connections)
 // connection-major (cm) pack path: dense messages with small records are grouped and written
 // connection by connection, so that one connection's records form ONE contiguous run in its ring
@@ -73,11 +75,11 @@ struct DevState {
   uint32_t N, W, T, nblk;
   uint32_t bucket_mask, key_stride;
   uint32_t ring_units;   // ring_bytes / 32
-  uint32_t fat_tile_bytes;  // bytes of stores per message-major pack tile
-  uint32_t fat_grab;        // consecutive message-major tiles a CTA takes per cursor update (A/B knob; 1 = default)
-  uint32_t cm_enable;    // connection-major pack class on (default) / off (A/B profiling)
   uint32_t n_valid_topics;  // Topic::prune validity bound (0 = all)
   uint32_t max_key_len;
+  uint64_t seed;
+  // (seed sits here so that the fields below keep their offsets: with them 12 bytes lower, k_offsets<false>
+  //  compiled to 40 registers instead of 32, i.e. 6 CTAs per SM instead of 8, and ran measurably slower)
   // connection shards (SURVEY 8e): this GPU owns the connection ids [conn_base, conn_base + N).  The
   // bitmap / broker-mask words here are this shard's slice (local word index); the direct map and
   // owner_conn[] are replicated on every shard and name connections by GLOBAL id, so a direct
@@ -95,7 +97,6 @@ struct DevState {
   uint32_t count_drops;  // 1 on exactly one shard of the broker (global shard 0): it counts the unroutable directs
   uint32_t shared_payload;  // PCDN_FLAG_SHARED_PAYLOAD: one 32-byte reference record per delivery (k_pack_ref), no cm class
   uint64_t ring_bytes;
-  uint64_t seed;
 };
 
 // inputs of one batch (device pointers) — same meaning as pcdn_device_batch
@@ -219,7 +220,7 @@ void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool 
                        BatchStats* publish, bool offsets_only, cudaStream_t st);
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);
-void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t variant, int n_sms, cudaStream_t st);
+void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms, cudaStream_t st);
 void launch_release(const DevState& s, const uint32_t* batch_units, const BatchStats* stats, cudaStream_t st);
 void launch_pool_init(const DevState& s, cudaStream_t st);
 unsigned long long kernel_launches();   // launches issued by this library in this process so far

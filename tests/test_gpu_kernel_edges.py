@@ -16,8 +16,7 @@ from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
 
-TILE_BYTES = 128 << 10   # message-major tile of the default configuration (engine.cu: DevState::fat_tile_bytes)
-REG_VECS = 128           # pack_fat_phase's st.global path keeps a chunk of up to 4 x 32 16-byte vectors in registers
+TILE_BYTES = K.kFatTileBytes   # bytes of stores a message-major tile aims at
 
 
 def vec_bytes(raw_len):
@@ -42,10 +41,8 @@ def edge_sizes():
     prefix moves the 16-byte vector and 32-byte unit steps)"""
     out = set()
     for b in (K.kCmMaxBytes - 4,                   # largest record on the connection-major path
-              REG_VECS * 16 - 4,                   # largest chunk the register path stores
               K.kChunkBytes - 4,                   # one staging chunk
-              2 * K.kChunkBytes - 4,               # two chunks
-              K.kChunkBytes + REG_VECS * 16 - 4):  # a second chunk at the register-path limit
+              2 * K.kChunkBytes - 4):              # two chunks
         out.update((b - 4, b - 1, b, b + 1, b + 4))
     return sorted(out)
 
@@ -103,21 +100,19 @@ def check(w):
     return n
 
 
-PACK_MODES = [(st, cm, out, ctrl) for st in ("tma", "st") for cm in ("cm", "no-cm") for out in ("rings", "pool")
-              for ctrl in ("fused", "regular")]
+PACK_MODES = [(out, ctrl) for out in ("rings", "pool") for ctrl in ("fused", "regular")]
 
 
-@pytest.mark.parametrize("st,cm,out,ctrl", PACK_MODES, ids=["-".join(m) for m in PACK_MODES])
-def test_pack_size_and_recipient_boundaries(pcdn, st, cm, out, ctrl):
+@pytest.mark.parametrize("out,ctrl", PACK_MODES, ids=["-".join(m) for m in PACK_MODES])
+def test_pack_size_and_recipient_boundaries(pcdn, out, ctrl):
     """every raw length of edge_sizes() to every recipient count of recipient_counts(): thin / fat / dense
-    (connection-major) classes, message-major tile edges, the register path of the st.global variant, the
-    staging-chunk edges; then connection-major groups of 7, 8, 9 and 17 records of the largest
-    connection-major size (8 of them fill the staging buffer exactly).  Recipients sit on the k_offsets
-    CTA, connection-major tile and match-block edges.  Small batches on a small engine take the fused
-    control kernel; FLAG_STAGED_SPANS forces the regular pipeline (k_pool_finish on 2 CTAs for the pool)."""
+    (connection-major) classes, message-major tile edges, the staging-chunk edges; then connection-major
+    groups of 7, 8, 9 and 17 records of the largest connection-major size (8 of them fill the staging
+    buffer exactly).  Recipients sit on the k_offsets CTA, connection-major tile and match-block edges.
+    Small batches on a small engine take the fused control kernel; FLAG_STAGED_SPANS forces the regular
+    pipeline (k_pool_finish on 2 CTAs for the pool)."""
     flags = (pcdn.FLAG_OUTPUT_POOL if out == "pool" else 0) | (pcdn.FLAG_STAGED_SPANS if ctrl == "regular" else 0)
-    variant = (4 if st == "st" else 0) | (2 if cm == "no-cm" else 0)
-    w, keys, topic = edge_world(pcdn, flags=flags, pack_variant=variant, pool_bytes=1 << 30)
+    w, keys, topic = edge_world(pcdn, flags=flags, pool_bytes=1 << 30)
     n = EDGE_SLOTS
     dense = n >> K.kCmDenseShift
     tag = 0
@@ -187,23 +182,19 @@ def test_direct_thresholds(pcdn):
 
 
 # ------------------------------------------------------------------ launch geometry
-# pack_variant A/B bits (kernels.cu launch_pack, engine.cu): 8-11 k_pack CTAs per SM, 12-15 k_pack_direct CTAs
-# per SM, 4-7 log2 message-major tile multiplier, 16-18 log2 tiles per cursor grab, 3 pack on the pack stream,
-# 5 never overlap broadcast batches (it also quadruples the tile), 2 st.global stores
+# pack_variant (kernels.cu launch_pack): bits 8-11 k_pack CTAs per SM, 12-15 k_pack_direct CTAs per SM
 GEOMETRY = {
     "pack-1cta": 1 << 8, "pack-2cta": 2 << 8, "pack-3cta": 3 << 8, "pack-4cta": 4 << 8, "pack-6cta": 6 << 8,
-    "pack-8cta": 8 << 8, "direct-1cta": 1 << 12, "direct-8cta": 8 << 12, "tile-x2": 1 << 4, "tile-x8": 3 << 4,
-    "grab-2": 1 << 16, "grab-8": 3 << 16, "pack-stream": 8, "no-overlap": 32, "st-1cta-grab8": 4 | 1 << 8 | 3 << 16,
+    "pack-8cta": 8 << 8, "direct-1cta": 1 << 12, "direct-8cta": 8 << 12,
 }
 
 
 @pytest.mark.parametrize("out", ["rings", "pool"])
-def test_launch_geometry_invariance(pcdn, out):
+def test_cta_count_invariance(pcdn, out):
     """one workload that reaches every pack phase — connection-major, message-major over several chunks,
     dense message-major, thin, >= kThinSeparateMin directs with a hot recipient, unknown keys, three
     batches so that the rings wrap — checked against ONE oracle run on the default engine and on engines
-    with other grid sizes, tile sizes, cursor grabs and streams: persistent-CTA phases must write the same
-    bytes whatever the grid."""
+    with other grid sizes: persistent-CTA phases must write the same bytes whatever the grid."""
     cfg = dict(ring_bytes_per_conn=1 << 18)
     if out == "pool":
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=1 << 28)

@@ -21,13 +21,6 @@ def test_reference_scenario_on_gpu(pcdn, scenario):
     scenario(EngineBackend(pcdn))
 
 
-@pytest.mark.parametrize("scenario", [scenarios.test_broadcast_user, scenarios.test_fifo_order],
-                         ids=lambda f: f.__name__)
-def test_reference_scenario_st_variant(pcdn, scenario):
-    """A/B variant: st.global.cs.v4 stores instead of TMA bulk stores"""
-    scenario(EngineBackend(pcdn, pack_variant=4))
-
-
 @pytest.mark.parametrize("scenario", scenarios.ALL, ids=lambda f: f.__name__)
 def test_reference_scenario_host_rings(pcdn, scenario):
     """egress hand-off mode (PCDN_FLAG_HOST_RINGS): the pack stores the framed records into mapped
@@ -163,8 +156,8 @@ def shard_cfg(pcdn, variant):
     return dict(devices=list(range(min(n, 4))), ingest=pcdn.INGEST_NCCL)
 
 
-@pytest.mark.parametrize("variant", [0, 4, 2, 8 + 65536, "staged", "runs", "runs-staged", "pool", "pool-st", "pool-staged-runs", "pool-host", "pool-shards", "pool-shards-nccl",
-                                     "pool-shards-staged", "host", "host-st", "shards-host", "shards-host-staged", "shards-nccl"])
+@pytest.mark.parametrize("variant", [0, "staged", "runs", "runs-staged", "pool", "pool-staged-runs", "pool-host", "pool-shards", "pool-shards-nccl",
+                                     "pool-shards-staged", "host", "shards-host", "shards-host-staged", "shards-nccl"])
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_random_mixed_batches(pcdn, seed, variant):
     """users + peer brokers, multi-topic broadcasts (fat and thin recipient sets), directs to local,
@@ -182,8 +175,6 @@ def test_random_mixed_batches(pcdn, seed, variant):
         # instead of per-connection rings
         fl = pcdn.FLAG_OUTPUT_POOL
         kw = {}
-        if variant == "pool-st":
-            kw["pack_variant"] = 4
         if variant == "pool-staged-runs":
             fl |= pcdn.FLAG_STAGED_SPANS | pcdn.FLAG_SPAN_RUNS
         if variant == "pool-host":
@@ -199,23 +190,18 @@ def test_random_mixed_batches(pcdn, seed, variant):
     elif variant in ("runs", "runs-staged"):
         # run-length span table (PCDN_FLAG_SPAN_RUNS): same streams, the table just arrives compressed
         w = World(pcdn, flags=pcdn.FLAG_SPAN_RUNS | (pcdn.FLAG_STAGED_SPANS if variant == "runs-staged" else 0), ring_bytes_per_conn=1 << 20)
-    elif variant in ("host", "host-st"):
+    elif variant == "host":
         # egress hand-off mode: rings in mapped pinned host memory, frames read in place by the host
-        # (TMA bulk stores / st.global.cs over PCIe)
-        w = World(pcdn, flags=pcdn.FLAG_HOST_RINGS, pack_variant=4 if variant == "host-st" else 0,
-                  ring_bytes_per_conn=1 << 20, max_conns=2048)
+        # (TMA bulk stores over PCIe)
+        w = World(pcdn, flags=pcdn.FLAG_HOST_RINGS, ring_bytes_per_conn=1 << 20, max_conns=2048)
         assert w.e.host_rings() != 0
     elif isinstance(variant, str):
         staged = variant.endswith("-staged")
         w = World(pcdn, ring_bytes_per_conn=1 << 20, max_conns=1024, flags=pcdn.FLAG_STAGED_SPANS if staged else 0,
                   **shard_cfg(pcdn, variant.removesuffix("-staged")))
         assert w.e.num_shards()[0] >= 2
-    elif variant == 8 + 65536:
-        # the pack on its own stream (overlaps the next batch's control kernels), forced onto the
-        # large-engine path where that stream is used
-        w = World(pcdn, pack_variant=8, flags=pcdn.FLAG_STAGED_SPANS, ring_bytes_per_conn=1 << 20)
     else:
-        w = World(pcdn, pack_variant=variant, ring_bytes_per_conn=1 << 20)
+        w = World(pcdn, ring_bytes_per_conn=1 << 20)
     keys = []
     for i in range(1500):
         k = rng.getrandbits(64).to_bytes(8, "little") * rng.choice([1, 4, 16])

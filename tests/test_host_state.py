@@ -340,3 +340,14 @@ def test_config_validation_of_round2_fields(pcdn):
     with pytest.raises(pcdn.PcdnError) as ei:
         e.retry_batch(1)
     assert ei.value.code == -3                               # host-only engine: no data path
+
+
+def test_pack_variant_takes_only_cta_counts(pcdn):
+    """pack_variant holds the CTAs per SM of k_pack (bits 8-11) and k_pack_direct (bits 12-15); every other
+    bit is refused with PCDN_EINVAL instead of being ignored"""
+    for bit in [*range(8), *range(16, 32)]:
+        with pytest.raises(pcdn.PcdnError) as ei:
+            pcdn.Engine(device=-1, max_conns=64, pack_variant=1 << bit)
+        assert ei.value.code == -1 and "CTA-count" in str(ei.value), bit
+    for v in (0, 3 << 8, 8 << 12, 0xFF00):
+        pcdn.Engine(device=-1, max_conns=64, pack_variant=v).close()
