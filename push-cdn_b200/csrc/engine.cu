@@ -1166,8 +1166,6 @@ int pcdn_handle_direct_message(pcdn_engine* e, const uint8_t* recipient, uint32_
 }
 
 // ---- frames to messages: user_receive_loop / broker_receive_loop (user/handler.rs, broker/handler.rs) ----
-static constexpr uint32_t kMaxWireTopics = 65536 / 8;
-
 // Device-parse engines without a hook for `origin`: a Direct or Broadcast frame is only tag-peeked
 // and copied; k_parse does the rest.  false: the frame takes the host parse.
 static bool devparse_msg(const pcdn_engine* e, uint32_t origin, const uint8_t* raw, uint32_t raw_len, InMsg* m) {
@@ -1183,13 +1181,13 @@ static bool devparse_msg(const pcdn_engine* e, uint32_t origin, const uint8_t* r
 // A parsed Direct or Broadcast frame as a message.  `f0` is its field 0 (the recipient or the wire topic
 // list; a hook may have replaced it).  Broker-origin messages go to users only; user-origin topic lists
 // are pruned (Topic::prune, user/handler.rs:133), broker-origin ones kept verbatim (handler.rs:157).
-// 0, or an error code and *why.
+// The wire list may be of any length: what counts against a batch is the entries it adds (n_topics),
+// which the admission rule (batch_limit) judges.  0, or an error code and *why.
 static int parsed_msg(const pcdn_engine* e, uint32_t origin, int kind, const uint8_t* raw, uint32_t raw_len,
                       const uint8_t* f0, uint32_t f0_len, InMsg* m, const char** why) {
   *m = InMsg{};
   m->kind = (uint8_t)kind; m->raw = raw; m->raw_len = raw_len; m->flags = origin ? MSGF_USERS_ONLY : 0;
   if (kind == PCDN_KIND_DIRECT) { m->key = f0; m->key_len = routed_key_len(e, f0_len); return 0; }
-  if (f0_len > kMaxWireTopics) { *why = "topic list too long"; return PCDN_EPARSE; }
   m->wire_topics = f0; m->n_listed = f0_len; m->prune = !origin;
   for (uint32_t t = 0; t < f0_len; t++) m->n_topics += !m->prune || topic_kept(f0, t, e->cfg.n_valid_topics) ? 1u : 0u;
   if (m->n_topics == 0 && m->prune) { *why = "supplied no valid topics"; return PCDN_EPRUNE; }
@@ -1246,15 +1244,14 @@ static int receive_locked(pcdn_engine* e, uint32_t origin, const uint8_t* sender
   }
   if (origin) return 1;
   if (pf.kind != PCDN_KIND_SUBSCRIBE && pf.kind != PCDN_KIND_UNSUBSCRIBE) return fail(PCDN_EKIND, "invalid message received");
-  uint16_t topics[kMaxWireTopics];
-  if (f0_len > kMaxWireTopics) return fail(PCDN_EPARSE, "topic list too long");
-  uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics);
+  std::vector<uint16_t> topics(f0_len);  // the wire list may be of any length, as in the reference
+  uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics.data());
   if (n == 0) return fail(PCDN_EPRUNE, "supplied no valid topics");
   int rc = before_state_change(e);
   if (rc) return rc;
   std::string key((const char*)sender, sender_len);
-  rc = pf.kind == PCDN_KIND_SUBSCRIBE ? e->conns->subscribe_user_to(key, topics, n)
-                                      : e->conns->unsubscribe_user_from(key, topics, n);
+  rc = pf.kind == PCDN_KIND_SUBSCRIBE ? e->conns->subscribe_user_to(key, topics.data(), n)
+                                      : e->conns->unsubscribe_user_from(key, topics.data(), n);
   return rc ? fail(rc, "topic id out of range") : 0;
 }
 
