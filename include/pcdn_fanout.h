@@ -504,12 +504,28 @@ int pcdn_poll_shard(pcdn_engine* e, uint64_t batch_id, uint32_t local_shard, pcd
  * whose send failed (cdn-broker/src/tasks/user/sender.rs:24-30).
  * PCDN_FLAG_SHARED_PAYLOAD: the chunks carry the reference records as stored; the fd sink sends each
  * as two iovecs (the 4 length bytes of the record, the L payload bytes from pcdn_batch_payload), and a
- * callback sink resolves them the same way through pcdn_batch_payload of the batch it drains.       */
+ * callback sink resolves them the same way through pcdn_batch_payload of the batch it drains.
+ * Backlogs (backlog_bytes_per_conn / backlog_bytes_total, opt-in): without them a socket that cannot
+ * take its bytes holds the fd sink in poll() for up to 30 s, and with it every other connection and
+ * the release of the batch.  With a backlog the fd sink never waits on a peer: sockets are written
+ * with MSG_DONTWAIT (other descriptors follow their own O_NONBLOCK mode), and on EAGAIN or a partial
+ * write the unsent bytes of that connection's records — wire bytes, also the payload bytes of
+ * reference records — are copied into a per-connection backlog in host memory.  The batch can be
+ * released as soon as pcdn_egress_write_batch returns.  A connection with a backlog gets one
+ * non-blocking attempt to flush it before its next records; whatever is left goes behind the backlog
+ * (per-connection order is kept).  Growing a backlog past backlog_bytes_per_conn, or all backlogs
+ * past backlog_bytes_total, is handled like a failed write: the connection is detached, its backlog
+ * dropped, and it is reported once by pcdn_egress_failed.  The host moves backlogs on with
+ * pcdn_egress_flush_backlog when their descriptors become writable (pcdn_egress_backlog lists them).*/
 typedef struct pcdn_egress pcdn_egress;
 typedef struct pcdn_egress_config {
-  uint32_t struct_size; /* = sizeof(pcdn_egress_config)                                              */
+  uint32_t struct_size; /* = sizeof(pcdn_egress_config); the size without the two backlog fields is
+                           accepted too and means "no backlog"                                        */
   uint32_t n_threads;   /* writer threads of the fd sink (0 = min(16, cores))                         */
   uint64_t chunk_bytes; /* pinned staging per chunk (0 = 64 MiB); 3 host + 2 device chunks per shard  */
+  uint64_t backlog_bytes_per_conn; /* bound of one connection's backlog (0 = only the total bounds it)  */
+  uint64_t backlog_bytes_total;    /* bound of all backlogs together (0 = only the per-connection bound);
+                                      both 0 = no backlog: the fd sink waits for slow peers (30 s bound) */
 } pcdn_egress_config;
 typedef struct pcdn_egress_chunk {
   uint32_t local_shard;
@@ -542,8 +558,17 @@ int pcdn_egress_write_batch(pcdn_egress* g, uint64_t batch_id, pcdn_egress_stats
 /* connections whose write failed since the last call (engine-owned array): the host removes them (R13) */
 int pcdn_egress_failed(pcdn_egress* g, const pcdn_conn** conns, uint32_t* n);
 /* Connection::soft_close protocols/mod.rs:287-306: launches the open batch, writes and RELEASES every
- * batch in flight (oldest first), then detaches `conn` and hands its descriptor back for closing.  */
+ * batch in flight (oldest first), writes the connection's backlog (waiting up to 30 s at a time for
+ * the peer), then detaches `conn` and hands its descriptor back for closing.  A write that fails on
+ * the way reports the connection (pcdn_egress_failed) and *fd_out is then -2.                       */
 int pcdn_egress_soft_close(pcdn_egress* g, pcdn_conn conn, int* fd_out);
+/* backlogs: write what the backlogged descriptors accept, polling them together for POLLOUT for up to
+ * timeout_ms (0 = one non-blocking pass; < 0 = until every backlog is written or failed).  A write
+ * error reports the connection as failed.  *n_pending (may be NULL) = connections still backlogged. */
+int pcdn_egress_flush_backlog(pcdn_egress* g, int timeout_ms, uint32_t* n_pending);
+/* the connections that have a backlog (engine-owned array, valid until the next egress call) and the
+ * bytes of all backlogs: the descriptors an event loop waits on for writability                      */
+int pcdn_egress_backlog(pcdn_egress* g, const pcdn_conn** conns, uint32_t* n, uint64_t* bytes);
 
 /* ---- introspection (tests, metrics: cdn-proto/src/connection/metrics.rs:12-28) ------------- */
 int pcdn_get_stats(pcdn_engine* e, pcdn_stats* out);

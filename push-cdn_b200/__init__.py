@@ -137,7 +137,11 @@ class ShardDesc(C.Structure):
 
 
 class EgressConfig(C.Structure):
-    _fields_ = [("struct_size", C.c_uint32), ("n_threads", C.c_uint32), ("chunk_bytes", C.c_uint64)]
+    _fields_ = [("struct_size", C.c_uint32), ("n_threads", C.c_uint32), ("chunk_bytes", C.c_uint64),
+                ("backlog_bytes_per_conn", C.c_uint64), ("backlog_bytes_total", C.c_uint64)]
+
+
+EGRESS_CONFIG_NO_BACKLOG_SIZE = EgressConfig.backlog_bytes_per_conn.offset   # struct_size of callers built before the backlog fields
 
 
 class EgressChunk(C.Structure):
@@ -241,6 +245,8 @@ ABI = {
     "pcdn_egress_write_batch": (_ci, [_vp, _u64, C.POINTER(EgressStats)]),
     "pcdn_egress_failed": (_ci, [_vp, C.POINTER(C.POINTER(_u32)), C.POINTER(_u32)]),
     "pcdn_egress_soft_close": (_ci, [_vp, _u32, C.POINTER(_ci)]),
+    "pcdn_egress_flush_backlog": (_ci, [_vp, _ci, C.POINTER(_u32)]),
+    "pcdn_egress_backlog": (_ci, [_vp, C.POINTER(C.POINTER(_u32)), C.POINTER(_u32), C.POINTER(_u64)]),
     "pcdn_get_stats": (_ci, [_vp, C.POINTER(Stats)]),
     "pcdn_set_timing": (_ci, [_vp, _ci]),
     "pcdn_ring_info": (_ci, [_vp, C.POINTER(_vp), C.POINTER(_u64), C.POINTER(_u32)]),
@@ -680,11 +686,16 @@ class Engine:
 class Egress:
     """The consumer of span tables (pcdn_egress_*): drains a batch's framed records into host memory
     chunk by chunk and hands them to a sink — a Python callback, or the built-in writev sink that
-    writes every connection's records to the file descriptor attached to it."""
+    writes every connection's records to the file descriptor attached to it.  With a backlog budget
+    (``backlog_bytes_per_conn`` / ``backlog_bytes_total``) that writer never waits for a slow peer:
+    what the peer does not take is kept in host memory and written by ``flush_backlog``."""
 
-    def __init__(self, engine: Engine, n_threads: int = 0, chunk_bytes: int = 0):
+    def __init__(self, engine: Engine, n_threads: int = 0, chunk_bytes: int = 0,
+                 backlog_bytes_per_conn: int = 0, backlog_bytes_total: int = 0,
+                 struct_size: Optional[int] = None):
         self.e, self.L = engine, engine.L
-        cfg = EgressConfig(C.sizeof(EgressConfig), n_threads, chunk_bytes)
+        cfg = EgressConfig(C.sizeof(EgressConfig) if struct_size is None else struct_size, n_threads, chunk_bytes,
+                           backlog_bytes_per_conn, backlog_bytes_total)
         h = C.c_void_p()
         engine._chk(self.L.pcdn_egress_create(engine.h, C.byref(cfg), C.byref(h)))
         self.h = h
@@ -740,3 +751,16 @@ class Egress:
         fd = C.c_int(-1)
         self.e._chk(self.L.pcdn_egress_soft_close(self.h, conn, C.byref(fd)))
         return fd.value
+
+    def flush_backlog(self, timeout_ms: int = 0) -> int:
+        """write what the backlogged descriptors accept (waiting up to timeout_ms; 0 = one pass, < 0 =
+        until all are written or failed); returns the number of connections still backlogged"""
+        n = C.c_uint32()
+        self.e._chk(self.L.pcdn_egress_flush_backlog(self.h, timeout_ms, C.byref(n)))
+        return n.value
+
+    def backlog(self) -> Tuple[List[int], int]:
+        """(connections with a backlog, bytes of all backlogs)"""
+        p, n, b = C.POINTER(C.c_uint32)(), C.c_uint32(), C.c_uint64()
+        self.e._chk(self.L.pcdn_egress_backlog(self.h, C.byref(p), C.byref(n), C.byref(b)))
+        return [p[i] for i in range(n.value)], b.value

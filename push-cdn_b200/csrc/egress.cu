@@ -14,6 +14,13 @@
 // padding between records skipped), on a small thread pool, keeping per-connection order.  On a
 // PCDN_FLAG_SHARED_PAYLOAD engine a reference record becomes two iovecs: its 4 length bytes and the L
 // bytes of the batch's payload (pcdn_batch_payload) it points to.
+//
+// With backlogs configured (pcdn_egress_config.backlog_bytes_*) the built-in sink never waits for a
+// peer: what a socket does not take is copied into that connection's backlog in host memory and
+// written later (before its next records, by pcdn_egress_flush_backlog, or by soft_close).  The
+// backlog is host memory rather than unreleased ring space because a ring is released per batch for
+// all its connections (k_release), the output pool frees a batch's region as a whole, and a shared
+// payload is freed when its batch is released: none of them can hold one slow connection's bytes.
 #include <errno.h>
 #include <poll.h>
 #include <sys/socket.h>
@@ -22,6 +29,7 @@
 
 #include <atomic>
 #include <condition_variable>
+#include <cstddef>
 #include <functional>
 
 #include "engine_internal.h"
@@ -134,6 +142,16 @@ struct Pool {
 
 inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
 
+// one connection's backlog (pcdn_egress_config.backlog_bytes_*): wire bytes its peer has not taken
+// yet, buf[head..).  Copies, never pointers: the chunk and the shared payload the bytes came from are
+// gone once the sink returns / the batch is released.
+struct Backlog {
+  std::vector<uint8_t> buf;
+  size_t head = 0;
+  bool listed = false;  // in pcdn_egress::bl_list
+  uint64_t pending() const { return buf.size() - head; }
+};
+
 }  // namespace
 
 struct pcdn_egress {
@@ -153,6 +171,15 @@ struct pcdn_egress {
   const uint8_t* payload = nullptr;
   uint64_t batch_id = 0;
   std::atomic<bool> bad_ref{false};
+  // backlogs (index = global connection id, allocated on a connection's first backlog).  During a
+  // drain only the writer-pool part that owns a connection touches its entry; the total is shared by
+  // every part of every shard thread.  bl_list: the connections with a backlog (a few stale entries
+  // whose backlog emptied are dropped under `mu`, where no drain runs).
+  bool backlog_on = false;
+  std::vector<std::unique_ptr<Backlog>> bl;
+  std::atomic<uint64_t> bl_total{0};
+  std::mutex bl_mu;  // bl_list during a drain
+  std::vector<pcdn_conn> bl_list, bl_out;
 };
 
 namespace {
@@ -344,6 +371,127 @@ bool write_all(int fd, struct iovec* iov, int cnt, uint64_t* nbytes, uint64_t* n
   return true;
 }
 
+// ---- backlogs: the fd sink never waits for a peer ---------------------------------------------
+// one write that does not wait: sockets with MSG_DONTWAIT whatever the descriptor's mode, other
+// descriptors as their O_NONBLOCK mode says.  Bytes written, 0 = the peer takes nothing now, -1 = error.
+ssize_t write_nowait(int fd, const struct iovec* iov, int cnt, bool* is_sock) {
+  for (;;) {
+    ssize_t w;
+    if (*is_sock) {
+      struct msghdr mh{};
+      mh.msg_iov = const_cast<struct iovec*>(iov); mh.msg_iovlen = (size_t)cnt;
+      w = ::sendmsg(fd, &mh, MSG_DONTWAIT | MSG_NOSIGNAL);
+      if (w < 0 && errno == ENOTSOCK) { *is_sock = false; continue; }
+    } else {
+      w = ::writev(fd, iov, cnt);
+    }
+    if (w >= 0) return w;
+    if (errno == EINTR) continue;
+    return (errno == EAGAIN || errno == EWOULDBLOCK) ? 0 : -1;
+  }
+}
+
+void drop_backlog(pcdn_egress* g, pcdn_conn c) {
+  if (g->bl.empty() || !g->bl[c]) return;
+  Backlog& b = *g->bl[c];
+  g->bl_total -= b.pending();
+  std::vector<uint8_t>().swap(b.buf);
+  b.head = 0;  // stays listed until the list is compacted
+}
+
+// a failed write: detach, drop the backlog, report once (sender.rs:24-30)
+void fail_conn(pcdn_egress* g, pcdn_conn c) {
+  g->fds[c] = -2;
+  drop_backlog(g, c);
+  std::lock_guard<std::mutex> lk(g->fail_mu);
+  g->failed.push_back(c);
+}
+
+// writes what the peer takes of a backlog now; false on a write error
+bool flush_nowait(pcdn_egress* g, int fd, Backlog& b, uint64_t* nbytes, uint64_t* nwrites) {
+  bool is_sock = true;
+  while (b.pending()) {
+    const struct iovec v{b.buf.data() + b.head, (size_t)b.pending()};
+    const ssize_t w = write_nowait(fd, &v, 1, &is_sock);
+    if (w < 0) return false;
+    if (w == 0) break;
+    (*nwrites)++;
+    *nbytes += (uint64_t)w;
+    b.head += (size_t)w;
+    g->bl_total -= (uint64_t)w;
+  }
+  if (!b.pending()) {
+    b.buf.clear(); b.head = 0;
+    if (b.buf.capacity() > (1u << 20)) std::vector<uint8_t>().swap(b.buf);
+  }
+  return true;
+}
+
+// copies iov[0..cnt) behind the connection's backlog; false when that would break a budget
+bool append_backlog(pcdn_egress* g, pcdn_conn c, const struct iovec* iov, int cnt) {
+  uint64_t add = 0;
+  for (int i = 0; i < cnt; i++) add += iov[i].iov_len;
+  if (!add) return true;
+  if (!g->bl[c]) g->bl[c].reset(new Backlog());
+  Backlog& b = *g->bl[c];
+  if (g->cfg.backlog_bytes_per_conn && b.pending() + add > g->cfg.backlog_bytes_per_conn) return false;
+  const uint64_t cap = g->cfg.backlog_bytes_total;
+  uint64_t cur = g->bl_total.load();
+  do {
+    if (cap && cur + add > cap) return false;
+  } while (!g->bl_total.compare_exchange_weak(cur, cur + add));
+  if (b.head && b.head >= b.buf.size() / 2) { b.buf.erase(b.buf.begin(), b.buf.begin() + (ptrdiff_t)b.head); b.head = 0; }
+  const uint64_t before = b.pending();
+  try {
+    for (int i = 0; i < cnt; i++) {
+      const uint8_t* p = (const uint8_t*)iov[i].iov_base;
+      b.buf.insert(b.buf.end(), p, p + iov[i].iov_len);
+    }
+  } catch (const std::bad_alloc&) {  // the bytes that did go in are dropped with the failed connection
+    g->bl_total -= add - (b.pending() - before);
+    return false;
+  }
+  if (!b.listed) {
+    b.listed = true;
+    std::lock_guard<std::mutex> lk(g->bl_mu);
+    g->bl_list.push_back(c);
+  }
+  return true;
+}
+
+// the fd sink's write with backlogs: older backlog first (one pass), then the span's records; what
+// the peer does not take goes behind the backlog.  false = the connection failed.
+bool write_or_queue(pcdn_egress* g, pcdn_conn c, int fd, struct iovec* iov, int cnt, uint64_t* nbytes, uint64_t* nwrites) {
+  if (Backlog* b = g->bl[c].get(); b && b->pending()) {
+    if (!flush_nowait(g, fd, *b, nbytes, nwrites)) return false;
+    if (b->pending()) return append_backlog(g, c, iov, cnt);  // per-connection FIFO (R9)
+  }
+  bool is_sock = true;
+  while (cnt > 0) {
+    const int take = std::min(cnt, 1024);  // IOV_MAX
+    const ssize_t w = write_nowait(fd, iov, take, &is_sock);
+    if (w < 0) return false;
+    if (w == 0) return append_backlog(g, c, iov, cnt);
+    (*nwrites)++;
+    *nbytes += (uint64_t)w;
+    size_t left = (size_t)w;
+    while (cnt > 0 && left >= iov->iov_len) { left -= iov->iov_len; iov++; cnt--; }
+    if (left && cnt > 0) { iov->iov_base = (uint8_t*)iov->iov_base + left; iov->iov_len -= left; }
+  }
+  return true;
+}
+
+// drops bl_list entries whose backlog emptied; only where no drain runs (under pcdn_egress::mu)
+void compact_backlog_list(pcdn_egress* g) {
+  size_t k = 0;
+  for (pcdn_conn c : g->bl_list) {
+    Backlog& b = *g->bl[c];
+    if (b.pending()) g->bl_list[k++] = c;
+    else b.listed = false;
+  }
+  g->bl_list.resize(k);
+}
+
 int fd_sink(void* user, const pcdn_egress_chunk* ch) {
   pcdn_egress* g = (pcdn_egress*)user;
   const uint32_t n = ch->n_spans;
@@ -381,12 +529,10 @@ int fd_sink(void* user, const pcdn_egress_chunk* ch) {
       }
       if (!ok) { g->bad_ref = true; continue; }   // a record of another batch: nothing of this span is written
       nrec += s.n_records;
-      if (!write_all(fd, iov.data(), (int)iov.size(), &nb, &nw)) {
-        // Err ⇒ the reference's sender removes the peer (tasks/user/sender.rs:24-30): report it, stop writing to it
-        g->fds[s.conn] = -2;
-        std::lock_guard<std::mutex> lk(g->fail_mu);
-        g->failed.push_back(s.conn);
-      }
+      const bool written = g->backlog_on ? write_or_queue(g, s.conn, fd, iov.data(), (int)iov.size(), &nb, &nw)
+                                         : write_all(fd, iov.data(), (int)iov.size(), &nb, &nw);
+      // Err ⇒ the reference's sender removes the peer (tasks/user/sender.rs:24-30): report it, stop writing to it
+      if (!written) fail_conn(g, s.conn);
     }
     g->fd_bytes += nb; g->fd_writes += nw; g->records += nrec; g->unattached += una;
   });
@@ -446,11 +592,17 @@ extern "C" {
 int pcdn_egress_create(pcdn_engine* e, const pcdn_egress_config* cfg, pcdn_egress** out) {
   GUARD_BEGIN
   if (!e || !out) return fail(PCDN_EINVAL, "null argument");
-  if (cfg && cfg->struct_size != sizeof(pcdn_egress_config)) return fail(PCDN_EINVAL, "pcdn_egress_config.struct_size mismatch (ABI)");
+  // callers built before the backlog fields pass the shorter struct: no backlog
+  constexpr uint32_t kNoBacklogSize = offsetof(pcdn_egress_config, backlog_bytes_per_conn);
+  if (cfg && cfg->struct_size != sizeof(pcdn_egress_config) && cfg->struct_size != kNoBacklogSize)
+    return fail(PCDN_EINVAL, "pcdn_egress_config.struct_size mismatch (ABI)");
   if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine has nothing to drain");
   pcdn_egress* g = new pcdn_egress();
   g->e = e;
-  if (cfg) g->cfg = *cfg;
+  if (cfg) std::memcpy(&g->cfg, cfg, cfg->struct_size);
+  g->cfg.struct_size = sizeof(pcdn_egress_config);
+  g->backlog_on = g->cfg.backlog_bytes_per_conn || g->cfg.backlog_bytes_total;
+  if (g->backlog_on) g->bl.resize(e->geo.N);
   if (!g->cfg.chunk_bytes) g->cfg.chunk_bytes = 64ull << 20;
   if (!(e->cfg.flags & PCDN_FLAG_OUTPUT_POOL)) g->cfg.chunk_bytes = std::max<uint64_t>(g->cfg.chunk_bytes, 2 * e->cfg.ring_bytes_per_conn);
   g->cfg.chunk_bytes = align_up(g->cfg.chunk_bytes, 4096);
@@ -486,12 +638,14 @@ int pcdn_egress_drain(pcdn_egress* g, uint64_t batch_id, pcdn_egress_sink sink, 
 int pcdn_egress_attach(pcdn_egress* g, pcdn_conn conn, int fd) {
   std::lock_guard<std::mutex> lk(g->mu);
   if (conn >= g->fds.size() || fd < 0) return fail(PCDN_EINVAL, "connection id or file descriptor out of range");
+  drop_backlog(g, conn);  // a reused connection id never inherits the bytes of an earlier peer
   g->fds[conn] = fd;
   return 0;
 }
 int pcdn_egress_detach(pcdn_egress* g, pcdn_conn conn) {
   std::lock_guard<std::mutex> lk(g->mu);
   if (conn >= g->fds.size()) return fail(PCDN_EINVAL, "connection id out of range");
+  drop_backlog(g, conn);
   g->fds[conn] = -1;
   return 0;
 }
@@ -535,8 +689,67 @@ int pcdn_egress_soft_close(pcdn_egress* g, pcdn_conn conn, int* fd_out) {
     if (rc) return rc;
     if ((rc = pcdn_release_batch(g->e, b))) return rc;
   }
+  // then the connection's backlog, waiting for the peer as the writer without backlogs does
+  if (const int fd = g->fds[conn]; fd >= 0 && g->backlog_on && g->bl[conn]) {
+    Backlog& b = *g->bl[conn];
+    uint64_t nb = 0, nw = 0;
+    bool ok = true;
+    while (ok && b.pending()) {
+      ok = flush_nowait(g, fd, b, &nb, &nw);
+      if (ok && b.pending()) {
+        struct pollfd p{fd, POLLOUT, 0};
+        const int r = ::poll(&p, 1, 30000);
+        ok = r > 0 || (r < 0 && errno == EINTR);
+      }
+    }
+    if (!ok) fail_conn(g, conn);
+    compact_backlog_list(g);
+  }
   if (fd_out) *fd_out = g->fds[conn];
   g->fds[conn] = -1;
+  return 0;
+  GUARD_END
+}
+
+int pcdn_egress_flush_backlog(pcdn_egress* g, int timeout_ms, uint32_t* n_pending) {
+  GUARD_BEGIN
+  std::lock_guard<std::mutex> lk(g->mu);
+  const auto t_end = std::chrono::steady_clock::now() + std::chrono::milliseconds(std::max(timeout_ms, 0));
+  std::vector<struct pollfd> pf;
+  for (;;) {
+    uint64_t nb = 0, nw = 0;
+    for (pcdn_conn c : g->bl_list) {
+      Backlog& b = *g->bl[c];
+      if (b.pending() && !flush_nowait(g, g->fds[c], b, &nb, &nw)) fail_conn(g, c);
+    }
+    compact_backlog_list(g);
+    if (g->bl_list.empty() || timeout_ms == 0) break;
+    int wait = -1;
+    if (timeout_ms > 0) {
+      const auto left = std::chrono::duration_cast<std::chrono::milliseconds>(t_end - std::chrono::steady_clock::now()).count();
+      if (left <= 0) break;
+      wait = (int)left;
+    }
+    pf.clear();
+    for (pcdn_conn c : g->bl_list) pf.push_back({g->fds[c], POLLOUT, 0});
+    const int r = ::poll(pf.data(), (nfds_t)pf.size(), wait);
+    if (r < 0 && errno != EINTR) return fail(PCDN_EINVAL, std::string("poll: ") + std::strerror(errno));
+    if (r == 0) break;
+  }
+  if (n_pending) *n_pending = (uint32_t)g->bl_list.size();
+  return 0;
+  GUARD_END
+}
+
+int pcdn_egress_backlog(pcdn_egress* g, const pcdn_conn** conns, uint32_t* n, uint64_t* bytes) {
+  GUARD_BEGIN
+  std::lock_guard<std::mutex> lk(g->mu);
+  compact_backlog_list(g);
+  g->bl_out = g->bl_list;
+  std::sort(g->bl_out.begin(), g->bl_out.end());
+  if (conns) *conns = g->bl_out.data();
+  if (n) *n = (uint32_t)g->bl_out.size();
+  if (bytes) *bytes = g->bl_total;
   return 0;
   GUARD_END
 }
