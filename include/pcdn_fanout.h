@@ -193,7 +193,23 @@ enum {
    *   bytes 24..31  zero
    * A writer walks a span as usual: at p, if BE32(p) == PCDN_REF_MARK it sends p[4..8) ‖ the L bytes at
    * payload + offset and advances 32 bytes; otherwise it handles a framed record as before.          */
-  PCDN_FLAG_SHARED_PAYLOAD = 32
+  PCDN_FLAG_SHARED_PAYLOAD = 32,
+  /* In-batch subscription changes.  Without this flag every subscription change launches the open
+   * batch first, so a receive window with k Subscribe / Unsubscribe frames becomes k + 1 batches.
+   * With it, pcdn_subscribe_user_to, pcdn_unsubscribe_user_from, pcdn_subscribe_broker_to,
+   * pcdn_unsubscribe_broker_from and a user's Subscribe / Unsubscribe frame on every receive path
+   * (after Topic::prune and the hook) become an EVENT of the open batch instead.  The event's position
+   * is the number of messages in the batch when it was recorded; it applies to exactly the batch's
+   * messages at or after that position and to every later batch, so each connection's delivered byte
+   * stream is identical to what the same calls produce without the flag: only batch boundaries differ.
+   * The host mirror changes at once (pcdn_debug_interested, pcdn_get_topic_sync see it immediately).
+   * Events are not messages: n_msgs, msg_status and the counters keep their meaning.
+   * An event that does not fit the open batch (max_batch_msgs events already, or its topics would
+   * overflow the descriptor block's topic entries) takes the path without the flag: the batch is
+   * launched, then the change is applied.  Prune errors stay synchronous (PCDN_EPRUNE / PCDN_EPARSE,
+   * no event).  Every other state call (add / remove of users and brokers, pcdn_apply_user_sync,
+   * pcdn_apply_topic_sync) still launches the open batch first.                                   */
+  PCDN_FLAG_INBATCH_SUBSCRIBE = 64
 };
 #define PCDN_REF_MARK 0xFFFFFFFFu
 

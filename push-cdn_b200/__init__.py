@@ -39,6 +39,7 @@ FLAG_OUTPUT_POOL = 16   # one shared output pool per GPU instead of a ring per c
 FLAG_SPAN_RUNS = 8      # run-length span table (BatchResult.runs): consecutive connections with identical spans
 FLAG_STAGED_SPANS = 2   # force the large-engine span path (table in HBM + D2H) on a small engine
 FLAG_SHARED_PAYLOAD = 32  # every delivery is one 32-byte reference record; the payload exists once per batch (batch_payload)
+FLAG_INBATCH_SUBSCRIBE = 64  # subscription changes become events of the open batch instead of launching it
 REF_MARK = 0xFFFFFFFF     # first 4 bytes of a reference record
 BATCH_READY = 1         # DeviceBatch.hints: the arrays are already complete in device memory
 INGEST_NCCL, INGEST_HOST = 0, 1   # sharded engines: NCCL broadcast over NVLink | every shard copies from host

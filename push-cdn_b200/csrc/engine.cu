@@ -54,9 +54,14 @@ int flush_journal(pcdn_engine* e) {
     } else {
       for (uint32_t i : t.dirty_sub) {
         const uint32_t row = i / W, wd = i % W;
-        if (wd >= w0 && wd < w0 + Ws) sh.h_u32.push_back(Upd32{0, row * Ws + (wd - w0), t.sub[i]});
+        if (wd >= w0 && wd < w0 + Ws) sh.h_u32.push_back(Upd32{0, row * Ws + (wd - w0), t.sub_upload(i)});
       }
     }
+    if (full_sub)   // words the open batch's events changed keep their value before the events (HostTables::hold)
+      for (const auto& h : t.held_sub) {
+        const uint32_t row = h.first / W, wd = h.first % W;
+        if (wd >= w0 && wd < w0 + Ws) sh.h_u32.push_back(Upd32{0, row * Ws + (wd - w0), h.second});
+      }
     for (uint32_t i : t.dirty_brk)
       if (i >= w0 && i < w0 + Ws) sh.h_u32.push_back(Upd32{1, i - w0, t.brk[i]});
     for (uint32_t i : t.dirty_owner) sh.h_u32.push_back(Upd32{2, i, t.owner_conn[i]});
@@ -103,7 +108,7 @@ int flush_journal(pcdn_engine* e) {
 void slot_reset_open(Slot& s) {
   s.arena_used = 0; s.n_direct = 0; s.devparse = false; s.ingress_bytes = 0; s.n_msgs = 0;
   s.kind.clear(); s.flags.clear(); s.slot_off16.clear(); s.raw_len.clear(); s.aux_off.clear(); s.aux_len.clear();
-  s.bcast_index.clear(); s.topics.clear();
+  s.bcast_index.clear(); s.topics.clear(); s.events.clear(); s.ev_topics.clear();
   s.device_input = false; s.counted = false;
 }
 
@@ -123,6 +128,7 @@ int acquire_open_slot(pcdn_engine* e) {
 void abandon_open(pcdn_engine* e) {
   if (e->open_slot < 0) return;
   Slot& s = e->slots[e->open_slot];
+  e->tables->release_held();   // its events' changes reach the device before the next batch
   e->inflight_bytes -= std::min(e->inflight_bytes, s.ingress_bytes);
   e->stats.bytes_in -= std::min(e->stats.bytes_in, s.ingress_bytes);
   slot_reset_open(s);
@@ -132,14 +138,16 @@ void abandon_open(pcdn_engine* e) {
 
 // Descriptor block of a batch: its per-message arrays at these offsets from the block's base (host-staged
 // batches, and device-resident ones as sharded engines replicate them)
+// (PCDN_FLAG_INBATCH_SUBSCRIBE: the subscription events and their topics follow the message topics)
 struct DescLayout {
-  uint32_t n_msgs, n_bcast;
-  size_t o_kind, o_flags, o_slot, o_len, o_aoff, o_alen, o_bidx, o_top, total;
-  DescLayout(uint32_t n, uint32_t nb, size_t n_topics) : n_msgs(n), n_bcast(nb) {
+  uint32_t n_msgs, n_bcast, n_events;
+  size_t o_kind, o_flags, o_slot, o_len, o_aoff, o_alen, o_bidx, o_top, o_ev, o_etop, total;
+  DescLayout(uint32_t n, uint32_t nb, size_t n_topics, uint32_t n_ev = 0, size_t n_ev_topics = 0) : n_msgs(n), n_bcast(nb), n_events(n_ev) {
     o_kind = 0; o_flags = align_up(o_kind + n, 16); o_slot = align_up(o_flags + n, 16);
     o_len = o_slot + (size_t)n * 4; o_aoff = o_len + (size_t)n * 4; o_alen = o_aoff + (size_t)n * 4;
     o_bidx = o_alen + (size_t)n * 4; o_top = align_up(o_bidx + (size_t)nb * 4, 16);
-    total = align_up(o_top + n_topics * 2, 16);
+    o_ev = align_up(o_top + n_topics * 2, 16); o_etop = o_ev + (size_t)n_ev * sizeof(SubEvent);
+    total = align_up(o_etop + n_ev_topics * 2, 16);
   }
 };
 
@@ -147,7 +155,8 @@ struct DescLayout {
 BatchIn bind_batch(const uint8_t* arena, const uint8_t* desc, const DescLayout& L) {
   return BatchIn{L.n_msgs, L.n_bcast, arena, desc + L.o_kind, desc + L.o_flags, (const uint32_t*)(desc + L.o_slot),
                  (const uint32_t*)(desc + L.o_len), (const uint32_t*)(desc + L.o_aoff), (const uint32_t*)(desc + L.o_alen),
-                 (const uint16_t*)(desc + L.o_top), (const uint32_t*)(desc + L.o_bidx)};
+                 (const uint16_t*)(desc + L.o_top), (const uint32_t*)(desc + L.o_bidx),
+                 L.n_events, (const SubEvent*)(desc + L.o_ev), (const uint16_t*)(desc + L.o_etop)};
 }
 
 // The adaptive pack-stream overlap applies to batches whose previous output was at most this many bytes.
@@ -399,11 +408,11 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
   const uint32_t si = (uint32_t)e->open_slot;
   Slot& s = e->slots[si];
   const uint32_t n = (uint32_t)s.kind.size();
-  if (n == 0) { abandon_open(e); return 0; }
+  if (n == 0) { abandon_open(e); return 0; }   // (events alone: no message sees them, they go up with the journal)
   if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
   int rc = flush_journal(e);
   if (rc) return rc;
-  const DescLayout L(n, (uint32_t)s.bcast_index.size(), s.topics.size());   // fits desc_cap (checked at create)
+  const DescLayout L(n, (uint32_t)s.bcast_index.size(), s.topics.size(), (uint32_t)s.events.size(), s.ev_topics.size());   // fits desc_cap (checked at create)
   // Small batches ride in ONE host→device copy: the descriptor block is appended to the frame arena
   // when it fits there (one DMA + one API call less on the latency path); otherwise two copies.
   // Sharded engines always use the appended layout: the batch is one ingest region.
@@ -418,6 +427,11 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
   std::memcpy(hd + L.o_alen, s.aux_len.data(), (size_t)n * 4);
   if (!s.bcast_index.empty()) std::memcpy(hd + L.o_bidx, s.bcast_index.data(), s.bcast_index.size() * 4);
   if (!s.topics.empty()) std::memcpy(hd + L.o_top, s.topics.data(), s.topics.size() * 2);
+  if (!s.events.empty()) {   // by (connection, position): the match finds a connection's events by binary search
+    std::stable_sort(s.events.begin(), s.events.end(), [](const SubEvent& a, const SubEvent& b) { return a.conn < b.conn; });
+    std::memcpy(hd + L.o_ev, s.events.data(), s.events.size() * sizeof(SubEvent));
+    std::memcpy(hd + L.o_etop, s.ev_topics.data(), s.ev_topics.size() * 2);
+  }
   if (e->sharded) {
     std::memset(s.h_arena + s.arena_used, 0, doff - s.arena_used);
     if ((rc = ingest_staged(e, si, s.h_arena, doff + L.total))) return rc;
@@ -437,7 +451,9 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
     ss.in = bind_batch(ss.d_arena, one_copy ? ss.d_arena + doff : ss.d_desc, L);
   }
   s.n_msgs = n;
-  if ((rc = launch_pipeline(e, si, e->sharded))) return rc;
+  rc = launch_pipeline(e, si, e->sharded);
+  e->tables->release_held();   // the events' words reach the device after this batch's control kernels
+  if (rc) return rc;
   if (batch_id) *batch_id = s.batch_id;
   return 0;
 }
@@ -445,7 +461,7 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
 // R12: a table mutation must not be visible to messages already handed to the engine
 int before_state_change(pcdn_engine* e) {
   int rc = 0;
-  if (e->open_slot >= 0 && !e->slots[e->open_slot].kind.empty()) rc = flush_open(e, nullptr);
+  if (e->open_slot >= 0 && (!e->slots[e->open_slot].kind.empty() || !e->slots[e->open_slot].events.empty())) rc = flush_open(e, nullptr);
   // connection-id quarantine (host_state.h): ids freed now may be named by spans of batches <= fence_now
   e->conns->fence_now = e->next_batch_id - 1;
   e->conns->oldest_unreleased = e->inflight.empty() ? ~0ull : e->inflight.front();
@@ -476,12 +492,15 @@ struct MsgShape {
 struct BatchFill {
   uint32_t msgs = 0, bcast = 0;
   uint64_t bytes = 0, topics = 0, ingress = 0;
+  uint64_t ev_topics = 0;   // topic entries of the batch's subscription events (they share the topic capacity)
   void add(const MsgShape& m) {
     msgs++; bcast += m.kind == PCDN_KIND_BROADCAST ? 1 : 0;
     bytes += m.bytes(); topics += m.n_topics; ingress += m.raw_len;
   }
 };
-BatchFill fill_of(const Slot& s) { return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0}; }
+BatchFill fill_of(const Slot& s) {
+  return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0, s.ev_topics.size()};
+}
 
 // The per-batch limits: nullptr when `m` still fits a batch that holds `f`, else the limit it would
 // break.  A message that does not fit an empty batch (BatchFill{}) never fits.
@@ -490,8 +509,63 @@ const char* batch_limit(const pcdn_engine* e, const BatchFill& f, const MsgShape
   if (f.msgs >= c.max_batch_msgs) return "max_batch_msgs";
   if (f.bytes + m.bytes() + 64 > c.max_batch_bytes) return "max_batch_bytes";
   if (m.kind == PCDN_KIND_BROADCAST && f.bcast >= c.max_batch_bcast) return "max_batch_bcast";
-  if (f.topics + m.n_topics > e->topics_cap) return "the topic entries of the descriptor block";
+  if (f.topics + f.ev_topics + m.n_topics > e->topics_cap) return "the topic entries of the descriptor block";
   return nullptr;
+}
+
+// ---- subscription changes -----------------------------------------------------------------------
+enum SubOp { SUB_USER, UNSUB_USER, SUB_BROKER, UNSUB_BROKER };
+
+// `op` on the mirror for the user key / broker identifier `who`; *conn: its connection (or NONE)
+int apply_sub(pcdn_engine* e, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n, uint32_t* conn) {
+  Connections& cn = *e->conns;
+  switch (op) {
+    case SUB_USER: *conn = cn.user_conn(who); return cn.subscribe_user_to(who, topics, n);
+    case UNSUB_USER: *conn = cn.user_conn(who); return cn.unsubscribe_user_from(who, topics, n);
+    case SUB_BROKER: *conn = cn.broker_conn(who.c_str()); return cn.subscribe_broker_to(who.c_str(), topics, n);
+    default: *conn = cn.broker_conn(who.c_str()); return cn.unsubscribe_broker_from(who.c_str(), topics, n);
+  }
+}
+
+// PCDN_FLAG_INBATCH_SUBSCRIBE: the open batch (opened here when there is none), holding `f`, takes one
+// more event of n topics
+bool event_fits(pcdn_engine* e, const BatchFill& f, uint32_t n) {
+  if (!(e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) || e->open_slot < 0) return false;
+  const Slot& s = e->slots[e->open_slot];
+  return s.events.size() < e->cfg.max_batch_msgs && f.topics + f.ev_topics + n <= e->topics_cap;
+}
+
+// `op` as an event of the open batch at position `pos`: the mirror changes now, the device bitmap keeps
+// the words' values before the batch's events until its control kernels have run (HostTables::hold), and
+// the batch's match replays the event on the messages at or after `pos` (kernels.cu: apply_events)
+int record_event(pcdn_engine* e, uint32_t pos, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n) {
+  HostTables& t = *e->tables;
+  Slot& s = e->slots[e->open_slot];
+  uint32_t conn;
+  t.hold = true;
+  const int rc = apply_sub(e, op, who, topics, n, &conn);
+  t.hold = false;
+  if (rc || conn == PCDN_CONN_NONE) return rc;   // (a connection not attached here changes no bit)
+  SubEvent ev{conn, pos | (op == SUB_USER || op == SUB_BROKER ? kEvSubscribe : 0u), (uint32_t)s.ev_topics.size(), 0};
+  for (uint32_t i = 0; i < n; i++)
+    if (topics[i] < e->geo.T) { s.ev_topics.push_back(topics[i]); ev.tn++; }   // (no other id has a bitmap row)
+  s.events.push_back(ev);
+  return 0;
+}
+
+// A subscription change from the C ABI or a user's Subscribe / Unsubscribe frame: an event of the open
+// batch when the flag is set and it fits there, else (R12) the open batch is launched first
+int sub_change(pcdn_engine* e, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n) {
+  int rc;
+  if ((e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) && (e->open_slot >= 0 || acquire_open_slot(e) == 0) &&
+      event_fits(e, fill_of(e->slots[e->open_slot]), n)) {
+    rc = record_event(e, (uint32_t)e->slots[e->open_slot].kind.size(), op, who, topics, n);
+  } else {
+    if ((rc = before_state_change(e))) return rc;
+    uint32_t conn;
+    rc = apply_sub(e, op, who, topics, n, &conn);
+  }
+  return rc ? fail(rc, "topic id out of range") : 0;
 }
 
 // a frame this engine never accepts (PCDN_EINVAL): the reason, else nullptr
@@ -853,7 +927,11 @@ int init_device(pcdn_engine* e) {
   const uint32_t M = c.max_batch_msgs;
   e->topics_cap = (size_t)M * 4 + 4096;
   e->desc_cap = align_up((size_t)M * 2 + 64, 16) + (size_t)M * 20 + 64 + e->topics_cap * 2 + 64;
-  if (DescLayout(M, std::min(M, c.max_batch_bcast), e->topics_cap).total > e->desc_cap)
+  // in-batch subscription events: up to max_batch_msgs of them; their topics share topics_cap
+  const uint32_t max_ev = (c.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) ? M : 0;
+  e->desc_cap += (size_t)max_ev * sizeof(SubEvent) + (max_ev ? 32 : 0);
+  if (DescLayout(M, std::min(M, c.max_batch_bcast), e->topics_cap, max_ev, 0).total > e->desc_cap ||
+      (max_ev && DescLayout(M, std::min(M, c.max_batch_bcast), 1, max_ev, e->topics_cap - 1).total > e->desc_cap))
     return fail(PCDN_EINVAL, "the descriptor block of a full batch exceeds desc_cap");
   // sharded engines keep frames + descriptor block in one ingest region (and device-input batches
   // need room for the descriptor arrays behind the frames)
@@ -1042,18 +1120,13 @@ int pcdn_remove_user(pcdn_engine* e, const uint8_t* key, uint32_t key_len) {
 int pcdn_subscribe_user_to(pcdn_engine* e, const uint8_t* key, uint32_t key_len, const uint16_t* topics, uint32_t n) {
   GUARD_BEGIN
   LOCK;
-  int rc = before_state_change(e);
-  if (rc) return rc;
-  rc = e->conns->subscribe_user_to(std::string((const char*)key, key_len), topics, n);
-  return rc ? fail(rc, "topic id out of range") : 0;
+  return sub_change(e, SUB_USER, std::string((const char*)key, key_len), topics, n);
   GUARD_END
 }
 int pcdn_unsubscribe_user_from(pcdn_engine* e, const uint8_t* key, uint32_t key_len, const uint16_t* topics, uint32_t n) {
   GUARD_BEGIN
   LOCK;
-  int rc = before_state_change(e);
-  if (rc) return rc;
-  return e->conns->unsubscribe_user_from(std::string((const char*)key, key_len), topics, n);
+  return sub_change(e, UNSUB_USER, std::string((const char*)key, key_len), topics, n);
   GUARD_END
 }
 int pcdn_add_broker(pcdn_engine* e, const char* identifier, pcdn_conn* out_conn) {
@@ -1076,18 +1149,13 @@ int pcdn_remove_broker(pcdn_engine* e, const char* identifier) {
 int pcdn_subscribe_broker_to(pcdn_engine* e, const char* identifier, const uint16_t* topics, uint32_t n) {
   GUARD_BEGIN
   LOCK;
-  int rc = before_state_change(e);
-  if (rc) return rc;
-  rc = e->conns->subscribe_broker_to(identifier, topics, n);
-  return rc ? fail(rc, "topic id out of range") : 0;
+  return sub_change(e, SUB_BROKER, std::string(identifier ? identifier : ""), topics, n);   // (BrokerIdent::parse reads null as "")
   GUARD_END
 }
 int pcdn_unsubscribe_broker_from(pcdn_engine* e, const char* identifier, const uint16_t* topics, uint32_t n) {
   GUARD_BEGIN
   LOCK;
-  int rc = before_state_change(e);
-  if (rc) return rc;
-  return e->conns->unsubscribe_broker_from(identifier, topics, n);
+  return sub_change(e, UNSUB_BROKER, std::string(identifier ? identifier : ""), topics, n);   // (BrokerIdent::parse reads null as "")
   GUARD_END
 }
 int pcdn_apply_user_sync(pcdn_engine* e, const char* remote_identity, const pcdn_user_sync_entry* entries, uint32_t n) {
@@ -1247,12 +1315,7 @@ static int receive_locked(pcdn_engine* e, uint32_t origin, const uint8_t* sender
   std::vector<uint16_t> topics(f0_len);  // the wire list may be of any length, as in the reference
   uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics.data());
   if (n == 0) return fail(PCDN_EPRUNE, "supplied no valid topics");
-  int rc = before_state_change(e);
-  if (rc) return rc;
-  std::string key((const char*)sender, sender_len);
-  rc = pf.kind == PCDN_KIND_SUBSCRIBE ? e->conns->subscribe_user_to(key, topics.data(), n)
-                                      : e->conns->unsubscribe_user_from(key, topics.data(), n);
-  return rc ? fail(rc, "topic id out of range") : 0;
+  return sub_change(e, pf.kind == PCDN_KIND_SUBSCRIBE ? SUB_USER : UNSUB_USER, std::string((const char*)sender, sender_len), topics.data(), n);
 }
 
 int pcdn_user_receive(pcdn_engine* e, const uint8_t* sender_key, uint32_t key_len, const uint8_t* raw, uint32_t raw_len) {
@@ -1273,11 +1336,12 @@ int pcdn_broker_receive(pcdn_engine* e, const char* identifier, const uint8_t* r
 extern "C++" {
 namespace {
 
-enum FrameRoute : int8_t { ROUTE_SEQUENTIAL, ROUTE_FAILED, ROUTE_BATCH };
+enum FrameRoute : int8_t { ROUTE_SEQUENTIAL, ROUTE_FAILED, ROUTE_BATCH, ROUTE_EVENT };
 // what the serial placement scan reads and writes per frame (kept small: the scan streams through it)
 struct FramePlan {
   // ROUTE_SEQUENTIAL: the frame goes through user/broker_receive_locked (state change, other kinds, a
-  // message no batch takes, which reports its error there); ROUTE_FAILED: protocol error `rc`
+  // message no batch takes, which reports its error there); ROUTE_FAILED: protocol error `rc`;
+  // ROUTE_EVENT (PCDN_FLAG_INBATCH_SUBSCRIBE): a user's Subscribe / Unsubscribe, recorded by the scan
   FrameRoute route;
   int32_t rc;
   MsgShape shape;
@@ -1314,9 +1378,13 @@ uint32_t ingest_threads() {
 //   B (parallel)  copy of the raw bytes into the pinned arena + descriptor fill by index
 // Frames that change state (Subscribe/Unsubscribe) or need the exact synchronous error path end a
 // run and go through user_receive_locked / broker_receive_locked, so R12 ordering is untouched.
+// PCDN_FLAG_INBATCH_SUBSCRIBE: a user's Subscribe / Unsubscribe is parsed and pruned in phase A and
+// becomes an event of the open batch in the scan (at its place among the messages); it ends the run
+// only when the batch cannot take the event.
 int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t* rc_out) {
   const pcdn_config& c = e->cfg;
   const uint32_t T = ingest_threads();
+  const bool inbatch = (c.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) != 0;
   // a hook sees every parsed message, in order
   const bool threaded = n >= 2048 && T > 1 && e->has_device && !e->hook[0] && !e->hook[1];
   // phase A writes every entry the later phases read
@@ -1331,11 +1399,23 @@ int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, 
       const uint32_t origin = f.origin ? 1 : 0;
       p.route = ROUTE_SEQUENTIAL; p.rc = 0;
       if (!devparse_msg(e, origin, f.raw, f.raw_len, &m)) {
-        if (c.flags & PCDN_FLAG_DEVICE_PARSE) continue;
+        const bool dp = (c.flags & PCDN_FLAG_DEVICE_PARSE) != 0, ev = inbatch && !origin;
+        if (dp && !ev) continue;
         ParsedFrame pf;
         const char* why;
-        if (!parse_frame(f.raw, f.raw_len, &pf)) { p.route = ROUTE_FAILED; p.rc = PCDN_EPARSE; continue; }
-        if (pf.kind != PCDN_KIND_DIRECT && pf.kind != PCDN_KIND_BROADCAST) continue;
+        if (!parse_frame(f.raw, f.raw_len, &pf)) {
+          if (!dp) { p.route = ROUTE_FAILED; p.rc = PCDN_EPARSE; }
+          continue;
+        }
+        if (ev && (pf.kind == PCDN_KIND_SUBSCRIBE || pf.kind == PCDN_KIND_UNSUBSCRIBE)) {
+          m = InMsg{};
+          m.kind = (uint8_t)pf.kind; m.wire_topics = f.raw + pf.f0_off; m.n_listed = pf.f0_len;
+          for (uint32_t t = 0; t < pf.f0_len; t++) m.n_topics += topic_kept(m.wire_topics, t, c.n_valid_topics) ? 1u : 0u;
+          if (m.n_topics) p.route = ROUTE_EVENT;
+          else { p.route = ROUTE_FAILED; p.rc = PCDN_EPRUNE; }
+          continue;
+        }
+        if (dp || (pf.kind != PCDN_KIND_DIRECT && pf.kind != PCDN_KIND_BROADCAST)) continue;
         p.rc = parsed_msg(e, origin, pf.kind, f.raw, f.raw_len, f.raw + pf.f0_off, pf.f0_len, &m, &why);
         if (p.rc) { p.route = ROUTE_FAILED; continue; }
       }
@@ -1365,10 +1445,23 @@ int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, 
       FramePlan& p = plan[j];
       if (p.route == ROUTE_FAILED) continue;
       if (p.route == ROUTE_SEQUENTIAL) break;
+      if (p.route == ROUTE_EVENT) {
+        const InMsg& m = msgs[j];
+        if (!event_fits(e, fill, m.n_topics)) { p.route = ROUTE_SEQUENTIAL; break; }   // launch, then the change
+        std::vector<uint16_t> topics(m.n_listed);
+        const uint32_t nt = prune_topics(m.wire_topics, m.n_listed, c.n_valid_topics, topics.data());
+        const pcdn_frame& f = frames[j];
+        p.rc = record_event(e, fill.msgs, m.kind == PCDN_KIND_SUBSCRIBE ? SUB_USER : UNSUB_USER,
+                            std::string((const char*)f.sender, f.sender_len), topics.data(), nt);
+        if (p.rc) fail(p.rc, "topic id out of range");
+        fill.ev_topics = s.ev_topics.size();
+        continue;
+      }
       if (batch_limit(e, fill, p.shape) || !pool_admits(e, fill.ingress + p.shape.raw_len)) { full = true; break; }
       p.msg_idx = fill.msgs; p.arena_off = fill.bytes; p.bcast_pos = fill.bcast; p.topic_off = (uint32_t)fill.topics;
       fill.add(p.shape);
     }
+    if (j == i && plan[i].route == ROUTE_SEQUENTIAL) continue;   // an event the open batch cannot take
     if (j == i) {  // nothing fits: the open batch is full (or the pool is) — launch it and retry, or give up
       if (s.kind.empty()) return i ? (int)i : fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
       if ((rc = flush_open(e, nullptr))) return i ? (int)i : rc;

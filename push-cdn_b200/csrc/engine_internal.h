@@ -143,6 +143,8 @@ struct Slot {
   std::vector<uint8_t> kind, flags;
   std::vector<uint32_t> slot_off16, raw_len, aux_off, aux_len, bcast_index;
   std::vector<uint16_t> topics;
+  std::vector<SubEvent> events;     // PCDN_FLAG_INBATCH_SUBSCRIBE: subscription events, in the order recorded
+  std::vector<uint16_t> ev_topics;  // ... and their topics
   uint32_t n_direct = 0;
   uint32_t n_msgs = 0;
   uint64_t ingress_bytes = 0;   // pool permits held by this batch

@@ -40,7 +40,15 @@ void HostTables::set_bit(uint32_t topic, uint32_t conn, bool on) {
   size_t i = (size_t)topic * g.W + (conn >> 5);
   uint32_t m = 1u << (conn & 31), old = sub[i];
   uint32_t nw = on ? (old | m) : (old & ~m);
-  if (nw != old) { sub[i] = nw; mark(dirty_sub, f_sub_, (uint32_t)i); }
+  if (nw != old) {
+    if (hold) held_sub.emplace((uint32_t)i, old);   // (keeps the value before the first change)
+    sub[i] = nw;
+    mark(dirty_sub, f_sub_, (uint32_t)i);
+  }
+}
+void HostTables::release_held() {
+  for (const auto& h : held_sub) mark(dirty_sub, f_sub_, h.first);
+  held_sub.clear();
 }
 bool HostTables::get_bit(uint32_t topic, uint32_t conn) const {
   return (sub[(size_t)topic * g.W + (conn >> 5)] >> (conn & 31)) & 1u;
@@ -216,6 +224,14 @@ int Connections::check_topics(const uint16_t* topics, uint32_t n) const {
 }
 bool Connections::has_broker(const char* ident) const {
   return brokers_.count(BrokerIdent::parse(ident).str()) != 0;
+}
+uint32_t Connections::user_conn(const std::string& key) const {
+  auto u = users_.find(key);
+  return u == users_.end() ? PCDN_CONN_NONE : u->second;
+}
+uint32_t Connections::broker_conn(const char* ident) const {
+  auto b = brokers_.find(BrokerIdent::parse(ident).str());
+  return b == brokers_.end() ? PCDN_CONN_NONE : b->second.conn;
 }
 
 // VersionedMap::modify_local versioned_map.rs:84-113

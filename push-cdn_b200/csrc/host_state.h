@@ -54,6 +54,18 @@ class HostTables {
   // dirty sets since the last take_*()
   std::vector<uint32_t> dirty_sub, dirty_brk, dirty_owner, dirty_slots, dirty_keys;
 
+  // In-batch subscription events (PCDN_FLAG_INBATCH_SUBSCRIBE): while `hold` is set, set_bit keeps the
+  // value a bitmap word had before its first change.  The device must keep that value while the batch
+  // that holds the events runs (its match replays the events per message); the held words' current
+  // values go up with the upload after it (release_held).
+  bool hold = false;
+  std::unordered_map<uint32_t, uint32_t> held_sub;   // word index → value before the open batch's events
+  uint32_t sub_upload(uint32_t i) const {             // what the next upload writes for dirty word i
+    auto it = held_sub.find(i);
+    return it == held_sub.end() ? sub[i] : it->second;
+  }
+  void release_held();
+
   void set_bit(uint32_t topic, uint32_t conn, bool on);
   bool get_bit(uint32_t topic, uint32_t conn) const;
   void set_broker(uint32_t conn, bool on);
@@ -151,6 +163,8 @@ class Connections {
   uint32_t shard_load(uint32_t shard) const { return shard < shard_load_.size() ? shard_load_[shard] : 0; }
   bool has_user(const std::string& key) const { return users_.count(key) != 0; }
   bool has_broker(const char* ident) const;
+  uint32_t user_conn(const std::string& key) const;   // PCDN_CONN_NONE when the user is not connected here
+  uint32_t broker_conn(const char* ident) const;      // PCDN_CONN_NONE when the broker is not connected
 
  private:
   struct VV { uint64_t version; bool has; uint32_t owner; };  // VersionedValue<BrokerIdentifier>

@@ -370,6 +370,68 @@ void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t 
 }
 
 // =============================================================================== K1a topic match
+// ---- in-batch subscription events (PCDN_FLAG_INBATCH_SUBSCRIBE).  The bitmap holds every connection's
+// membership as it was when the batch was opened; a connection with events gets its bit of message m
+// re-evaluated: per topic of m, its membership before the batch with its events at positions <= m
+// replayed in order, ORed over the topics.  Both match paths patch their words before the popcounts, so
+// ranks, plan, offsets and pack see the patched bits like any other.
+
+// topic i of message m's list (toff, fl: m's aux_off, flags): false when Topic::prune drops it or it names no row
+__device__ __forceinline__ bool msg_topic(const DevState& s, const BatchIn& b, uint32_t fl, uint32_t toff, uint32_t i, uint32_t* t) {
+  if (fl & MSGF_TOPICS_U8) {
+    const uint8_t* tb = b.arena + toff;
+    if ((fl & MSGF_PRUNE) && !topic_kept(tb, i, s.n_valid_topics)) return false;
+    *t = tb[i];
+  } else {
+    *t = b.topics[toff + i];
+  }
+  return *t < s.T;
+}
+
+// bit k of local word wd for message m, with the connection's events [e0, e1) (its events at positions <= m)
+__device__ uint32_t event_bit(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd, uint32_t k, uint32_t e0, uint32_t e1) {
+  const uint32_t fl = b.flags[m], toff = b.aux_off[m], tn = b.aux_len[m];
+  for (uint32_t i = 0; i < tn; i++) {
+    uint32_t t;
+    if (!msg_topic(s, b, fl, toff, i, &t)) continue;
+    uint32_t on = (s.sub[(size_t)t * s.W + wd] >> k) & 1u;
+    for (uint32_t e = e0; e < e1; e++) {
+      const SubEvent ev = b.events[e];
+      for (uint32_t q = 0; q < ev.tn; q++)
+        if (b.ev_topics[ev.toff + q] == t) { on = ev.pos_op >> 31; break; }
+    }
+    if (on) return 1u;
+  }
+  return 0u;
+}
+
+// patch NW consecutive match words v[] of message m, the first at local word wd0: one binary search for
+// the first event of these 32 * NW connections, then the events of those connections only
+template <int NW>
+__device__ __forceinline__ void apply_events(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd0, uint32_t* v) {
+  const uint32_t ne = b.n_events, c_lo = s.conn_base + wd0 * 32, c_hi = c_lo + NW * 32;
+  uint32_t e = 0, hi = ne;
+  while (e < hi) {
+    const uint32_t mid = (e + hi) >> 1;
+    if (b.events[mid].conn < c_lo) e = mid + 1; else hi = mid;
+  }
+  while (e < ne) {
+    const uint32_t c = b.events[e].conn;
+    if (c >= c_hi) break;
+    uint32_t e1 = e;   // c's events at positions <= m
+    while (e1 < ne && b.events[e1].conn == c && (b.events[e1].pos_op & ~kEvSubscribe) <= m) e1++;
+    if (e1 > e) {
+      const uint32_t q = (c - c_lo) >> 5, k = c & 31u;   // (c_lo is a multiple of 32)
+      const uint32_t bit = event_bit(s, b, m, wd0 + q, k, e, e1);
+#pragma unroll
+      for (int x = 0; x < NW; x++)
+        if ((uint32_t)x == q) v[x] = (v[x] & ~(1u << k)) | (bit << k);
+    }
+    while (e1 < ne && b.events[e1].conn == c) e1++;   // c's later events
+    e = e1;
+  }
+}
+
 // match word `wd` (32 connections) of message m: OR of its topics' bitmap rows (a2)
 __device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd) {
   const uint32_t toff = b.aux_off[m], tn = b.aux_len[m];
@@ -388,12 +450,14 @@ __device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn&
       if (t < s.T) word |= s.sub[(size_t)t * s.W + wd];
     }
   }
+  if (b.n_events) apply_events<1>(s, b, m, wd, &word);
   if (fl & MSGF_USERS_ONLY) word &= ~s.brk[wd];  // to_users_only (connections/mod.rs:111)
   return word;
 }
 // Warp = one 256-word match block of one message, lane = 8 consecutive words (32-byte vector
 // loads of the bitmap rows, no block-level synchronisation: the popcount prefix of a 256-word block
 // is a lane-local prefix plus one warp scan).  grid = (ceil(nblk / 8), n_bcast).
+template <bool EVENTS>
 __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w) {
   const uint32_t j = blockIdx.y, lane = lane_id();
   const uint32_t blk = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -417,6 +481,11 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w) {
     }
   } else {
     for (uint32_t i = 0; i < tn; i++) or_row(b.topics[toff + i]);
+  }
+  if (EVENTS) {
+    uint32_t v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    apply_events<8>(s, b, m, w0, v);
+    lo = make_uint4(v[0], v[1], v[2], v[3]); hi = make_uint4(v[4], v[5], v[6], v[7]);
   }
   if (fl & MSGF_USERS_ONLY) {  // to_users_only (connections/mod.rs:111)
     const uint4* br = reinterpret_cast<const uint4*>(s.brk + w0);
@@ -458,7 +527,10 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w) {
 void launch_match(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st) {
   if (!b.n_bcast) return;
   dim3 grid((s.nblk + 7) / 8, b.n_bcast);
-  PCDN_COUNT_LAUNCH, k_match<<<grid, 256, 0, st>>>(s, b, w);
+  // (a batch with in-batch subscription events takes its own instantiation: the one without them keeps
+  //  the registers and occupancy it has without the patch)
+  if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true><<<grid, 256, 0, st>>>(s, b, w);
+  else PCDN_COUNT_LAUNCH, k_match<false><<<grid, 256, 0, st>>>(s, b, w);
 }
 
 // =============================================================================== K1p plan

@@ -8,6 +8,7 @@
 //                       connection's segment (no sort: the connection's thread orders its few entries
 //                       in k_offsets; k_dsort_hot orders connections with > 32 hits by bitmap)
 //   K1a k_match         OR of subscription-bitmap rows per broadcast → match words + popcount ranks
+//                       (bits of connections with in-batch subscription events re-evaluated per message)
 //   K1p k_plan_*        D_m per message, class (thin / message-major / connection-major), scatter-list
 //                       bases and pack tiles by prefix sums (one launch when <= 256 messages)
 //   K1b k_offsets       thread per connection walks the batch IN ORDER (R9), assigns ring offsets and
@@ -99,6 +100,17 @@ struct DevState {
   uint64_t ring_bytes;
 };
 
+// PCDN_FLAG_INBATCH_SUBSCRIBE: a subscription change recorded inside a batch.  It applies to the batch's
+// messages at index >= position; the match of every other message reads the bitmap as it was when the
+// batch was opened.  Events are sorted by (conn, position), so a connection's events are one run.
+struct SubEvent {
+  uint32_t conn;     // global connection id
+  uint32_t pos_op;   // bits 0..30: position (messages in the batch when it was recorded); bit 31: 1 = subscribe
+  uint32_t toff;     // first topic in the batch's event topic list (u16 each)
+  uint32_t tn;       // topics
+};
+constexpr uint32_t kEvSubscribe = 0x80000000u;
+
 // inputs of one batch (device pointers) — same meaning as pcdn_device_batch
 struct BatchIn {
   uint32_t n_msgs, n_bcast;
@@ -111,6 +123,10 @@ struct BatchIn {
   const uint32_t* aux_len;
   const uint16_t* topics;
   const uint32_t* bcast_index;
+  // in-batch subscription events (0 unless PCDN_FLAG_INBATCH_SUBSCRIBE)
+  uint32_t n_events;
+  const SubEvent* events;
+  const uint16_t* ev_topics;
 };
 
 struct BatchStats {
