@@ -539,7 +539,6 @@ def main():
         "deliveries_per_step": int(d), "direct_dropped_per_step": int(dropped),
         "algorithmic_GBps": ab / step_s / 1e9, "frac_of_hbm_peak": ab / step_s / 1e9 / peak,
         "config": dict(desc, setup_s=round(setup_s, 1), pack_variant=args.variant),
-        # (ms_pack is 0 when the stage events went to the PCDN_TIMELINE_ASYNC dump instead of the engine's stage counters)
         "roofline": {"bound": "hbm", "kernel": "k_pack", "achieved": pack_bytes / (st["ms_pack"] * 1e-3) / 1e9 if st["ms_pack"] else None, "peak": peak, "unit": "GB/s",
                      "frac": pack_bytes / (st["ms_pack"] * 1e-3) / 1e9 / peak if st["ms_pack"] else None, "peak_source": peak_src, "stage_ms": st},
         "clocks": clocks,

@@ -588,11 +588,9 @@ int pcdn_egress_backlog(pcdn_egress* g, const pcdn_conn** conns, uint32_t* n, ui
 
 /* ---- introspection (tests, metrics: cdn-proto/src/connection/metrics.rs:12-28) ------------- */
 int pcdn_get_stats(pcdn_engine* e, pcdn_stats* out);
-/* the per-stage device times of the stats struct (ms_direct .. ms_pack) are accumulated while this is on.
- * Diagnostic, environment only: PCDN_TIMELINE=<file> appends one line per batch with the device
- * timestamps of its stage events (written when the batch is released, which then blocks until its
- * pack is done; with PCDN_TIMELINE_ASYNC=1 nothing blocks and the last 64 batches are written when
- * the engine is destroyed). */
+/* the per-stage device times of the stats struct (ms_direct .. ms_pack) are accumulated while this is on:
+ * CUDA events around the stages of the first local shard, read when the batch is polled.  Per-kernel
+ * timestamps come from a profiler (e.g. torch.profiler with CUDA activities) in a run of its own. */
 int pcdn_set_timing(pcdn_engine* e, int on);
 /* device pointer + geometry of the rings (zero-copy verification / GPUDirect hand-off) */
 int pcdn_ring_info(pcdn_engine* e, void** dev_base, uint64_t* ring_bytes, uint32_t* max_conns);

@@ -163,7 +163,6 @@ BatchIn bind_batch(const uint8_t* arena, const uint8_t* desc, const DescLayout& 
 // With every step queued ahead, overlapped packs can lose the launch race against the next control stage
 // and run much longer; the overlap hides at most the short control stage, so it stops paying for long packs.
 static constexpr unsigned long long kOverlapMaxBytes = 3ull << 29;
-static constexpr uint32_t kTimelineBatches = 64;
 
 // run the kernel pipeline of one shard for slot `si`, whose BatchIn is ready (or will be, once
 // ev_ingest fires) in that shard's memory.
@@ -202,15 +201,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   cudaStream_t st = sh.stream, ps = (!dp && (direct_only || fat_overlap)) ? sh.pack_stream : sh.stream, cs = sh.copy_stream;
   const bool has_direct = n_direct > 0;
   if (wait_ingest) CUDA_TRY(cudaStreamWaitEvent(st, s.ev_ingest, 0));
-  s.timed = e->timing && !e->timeline_async;
-  cudaEvent_t* tev = s.ev;
-  bool timed = s.timed;
-  if (e->timeline_async) {   // diagnostic: stage events from a ring of kTimelineBatches sets, read back when the engine goes away
-    const uint32_t k = sh.tl_n++ % kTimelineBatches;
-    tev = &sh.tl_ev[(size_t)k * 6];
-    sh.tl_batch[k] = e->next_batch_id;
-    timed = true;
-  }
+  s.timed = e->timing;
   s.polled = false;
   s.n_msg_errors = 0;
   // validity stamp of this batch's direct buckets / look-back words (a retry keeps it: the fused
@@ -237,7 +228,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   s.w.spans = s.spans_mapped ? s.d_spans_map : s.d_spans_dev;
   s.w.overflow = s.spans_mapped ? s.d_ovf_map : s.d_ovf_dev;
   const bool zero_in_kernel = fused && !devparse && !retry;  // (k_parse counts into the batch counters before the fused kernel)
-  if (timed) CUDA_TRY(cudaEventRecord(tev[0], st));
+  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[0], st));
   if (retry) {
     launch_pool_retry_begin(sh.dev, s.w, st);
   } else {
@@ -245,16 +236,16 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
     if (devparse) launch_parse(sh.dev, s.w, s.in, st);
     if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
   }
-  if (timed) CUDA_TRY(cudaEventRecord(tev[1], st));
+  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[1], st));
   if (fused) {
     launch_ctrl_small(sh.dev, s.w, s.in, has_direct, zero_in_kernel, s.d_stats_pub, retry, st);
-    if (timed) { CUDA_TRY(cudaEventRecord(tev[2], st)); CUDA_TRY(cudaEventRecord(tev[3], st)); }
+    if (s.timed) { CUDA_TRY(cudaEventRecord(s.ev[2], st)); CUDA_TRY(cudaEventRecord(s.ev[3], st)); }
   } else {
     if (!retry) launch_match(sh.dev, s.w, s.in, st);
-    if (timed) CUDA_TRY(cudaEventRecord(tev[2], st));
+    if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[2], st));
     if (!retry) launch_plan(sh.dev, s.w, s.in, st);
     launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);   // pool mode: a pure function of the scratch
-    if (timed) CUDA_TRY(cudaEventRecord(tev[3], st));
+    if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[3], st));
   }
   if (!s.spans_mapped) {
     CUDA_TRY(cudaEventRecord(s.ev_ctrl, st));
@@ -267,16 +258,14 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   }
   // (mapped spans: k_offsets wrote spans / overflow into host memory; everything stays on one
   //  stream and the host waits for ev_done only)
-  s.on_pack_stream = ps != st;
-  if (e->timeline_async) sh.tl_ps[(sh.tl_n - 1) % kTimelineBatches] = (int)s.on_pack_stream;
-  if (timed) CUDA_TRY(cudaEventRecord(tev[4], ps));
+  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[4], ps));
   // k_pack CTAs per SM unless pack_variant bits 8-11 set them: 4 when the pack has the GPU to itself, 3 when it
   // overlaps the next batch's control kernels (one H100: C2 +1.4 % with 4; the overlapped config-5 sparse shard
   // +2 % with 3)
   uint32_t pack_variant = e->cfg.pack_variant;
   if (!((pack_variant >> 8) & 15u)) pack_variant |= (fat_overlap ? 3u : 4u) << 8;
   launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, ps);
-  if (timed) CUDA_TRY(cudaEventRecord(tev[5], ps));
+  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[5], ps));
   CUDA_TRY(cudaGetLastError());
   if (!fused) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));
   CUDA_TRY(cudaEventRecord(s.ev_done, ps));
@@ -301,66 +290,37 @@ int launch_pipeline(pcdn_engine* e, uint32_t si, bool wait_ingest) {
   return 0;
 }
 
-// Sharded engines: bring `bytes` of slot si's pinned staging (or, for device input, `src_root` on the
-// root GPU) into every shard's d_arena.  NCCL mode: H2D on the root's ingest stream, then ONE
-// ncclBroadcast per region over all shards of the broker (grouped over the local shards), all on the
-// ingest streams — ahead of the main streams, so it overlaps the pack of the previous batch.  The
-// region may only be overwritten once the pack that last read this slot's arena is done (ev_done).
-struct IngestRegion { const void* root_src; size_t dst_off; size_t bytes; };  // root_src: device pointer on the root, or nullptr = staged bytes
-// Host-staged batch: `bytes` of slot si's pinned staging → every shard's d_arena.
-int ingest_staged(pcdn_engine* e, uint32_t si, const uint8_t* h_src, size_t bytes) {
-  if (e->ingest == PCDN_INGEST_HOST) {   // every shard copies from the pinned staging itself
-    for (Shard& sh : e->shards) {
-      DeviceGuard dg(sh.device);
-      ShardSlot& ss = sh.slots[si];
-      CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, ss.ev_done, 0));
-      CUDA_TRY(cudaMemcpyAsync(ss.d_arena, h_src, bytes, cudaMemcpyHostToDevice, sh.ingest_stream));
-      CUDA_TRY(cudaEventRecord(ss.ev_ingest, sh.ingest_stream));
-    }
-    return 0;
-  }
-  const NcclApi* nc = e->nccl;
-  for (Shard& sh : e->shards) {
-    DeviceGuard dg(sh.device);
-    ShardSlot& ss = sh.slots[si];
-    CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, ss.ev_done, 0));
-    if (sh.gindex == 0) CUDA_TRY(cudaMemcpyAsync(ss.d_arena, h_src, bytes, cudaMemcpyHostToDevice, sh.ingest_stream));
-  }
-  NCCL_TRY(nc, nc->GroupStart());
-  for (Shard& sh : e->shards) {
-    DeviceGuard dg(sh.device);
-    ShardSlot& ss = sh.slots[si];
-    int rc = nc->Broadcast(ss.d_arena, ss.d_arena, bytes, kNcclUint8, 0, sh.comm, sh.ingest_stream);
-    if (rc) { nc->GroupEnd(); return fail(PCDN_ECUDA, std::string("ncclBroadcast: ") + nc->GetErrorString(rc)); }
-  }
-  NCCL_TRY(nc, nc->GroupEnd());
-  for (Shard& sh : e->shards) {
-    DeviceGuard dg(sh.device);
-    CUDA_TRY(cudaEventRecord(sh.slots[si].ev_ingest, sh.ingest_stream));
-  }
-  return 0;
-}
-
-// Device-resident batch (its arrays lie on the root GPU, global shard 0).  The root first GATHERS the
-// descriptor arrays — and the frames too unless they are large (`arena_in_place`) — into its own slot
-// region with a few device-to-device copies, so that ONE ncclBroadcast of one contiguous range (two
-// with in-place frames) replicates the batch; nine separate broadcasts per step cost C5-sparse 8 % at
-// 8 GPUs.  `wait_submit`: order the ingest after everything queued on the root's main stream (the
-// caller's producer kernels); false when the caller says the buffers are already complete, so the
-// broadcast of batch n+1 overlaps the pack of batch n.
-int ingest_device(pcdn_engine* e, uint32_t si, const IngestRegion* regs, int nregs, bool arena_in_place, bool wait_submit) {
-  // regs[0] = frames at offset 0, regs[1..] = descriptor arrays behind them (ascending dst_off)
-  const size_t desc_lo = regs[1].dst_off, all_hi = regs[nregs - 1].dst_off + regs[nregs - 1].bytes;
-  if (e->ingest == PCDN_INGEST_HOST) {   // single process: peer copies from the root's buffers; the root reads in place
+// Sharded engines: bring a batch into every shard's d_arena, on the ingest streams — ahead of the main
+// streams, so that it overlaps the pack of the previous batch.  The region may only be overwritten once
+// the pack that last read this slot's arena is done (ev_done).  `regs`: the batch's pieces, regs[0] = the
+// frames at offset 0, the descriptor block behind them (ascending dst_off).
+//  - host-staged batch: one region, the slot's pinned staging (frames + descriptor block);
+//  - device-resident batch (its arrays lie on the root GPU, global shard 0): the frames and the eight
+//    descriptor arrays.  The root first GATHERS the descriptor arrays — and the frames too unless they are
+//    large (`arena_in_place`) — into its own slot region with a few device-to-device copies, so that ONE
+//    ncclBroadcast of one contiguous range (two with in-place frames) replicates the batch; nine separate
+//    broadcasts per step cost C5-sparse 8 % at 8 GPUs.
+// PCDN_INGEST_HOST (single process): every shard copies the regions itself (peer copies from the root's
+// buffers).  PCDN_INGEST_NCCL: the root copies them, then ncclBroadcast over all shards of the broker
+// (grouped over the local shards).  `wait_submit`: order the ingest after everything queued on the root's
+// main stream (the caller's producer kernels); false when the caller says the buffers are already
+// complete, so the broadcast of batch n+1 overlaps the pack of batch n.
+struct IngestRegion { const void* src; size_t dst_off; size_t bytes; bool host = false; };  // src: pinned host memory, or device memory of the root
+int ingest_batch(pcdn_engine* e, uint32_t si, const IngestRegion* regs, int nregs, bool arena_in_place, bool wait_submit) {
+  const size_t all_hi = regs[nregs - 1].dst_off + regs[nregs - 1].bytes;
+  if (e->ingest == PCDN_INGEST_HOST) {
     for (Shard& sh : e->shards) {
       DeviceGuard dg(sh.device);
       ShardSlot& ss = sh.slots[si];
       CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, ss.ev_done, 0));
       if (wait_submit) CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, e->shards[0].ev_submit, 0));
       for (int r = 0; r < nregs; r++) {
-        if (!regs[r].bytes || (sh.gindex == 0 && r == 0 && arena_in_place)) continue;
-        if (sh.gindex == 0) CUDA_TRY(cudaMemcpyAsync(ss.d_arena + regs[r].dst_off, regs[r].root_src, regs[r].bytes, cudaMemcpyDeviceToDevice, sh.ingest_stream));
-        else CUDA_TRY(cudaMemcpyPeerAsync(ss.d_arena + regs[r].dst_off, sh.device, regs[r].root_src, e->shards[0].device, regs[r].bytes, sh.ingest_stream));
+        const IngestRegion& g = regs[r];
+        if (!g.bytes || (sh.gindex == 0 && r == 0 && arena_in_place)) continue;
+        if (g.host || sh.gindex == 0)
+          CUDA_TRY(cudaMemcpyAsync(ss.d_arena + g.dst_off, g.src, g.bytes, g.host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, sh.ingest_stream));
+        else
+          CUDA_TRY(cudaMemcpyPeerAsync(ss.d_arena + g.dst_off, sh.device, g.src, e->shards[0].device, g.bytes, sh.ingest_stream));
       }
       CUDA_TRY(cudaEventRecord(ss.ev_ingest, sh.ingest_stream));
     }
@@ -373,18 +333,21 @@ int ingest_device(pcdn_engine* e, uint32_t si, const IngestRegion* regs, int nre
     CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, ss.ev_done, 0));
     if (sh.gindex != 0) continue;
     if (wait_submit) CUDA_TRY(cudaStreamWaitEvent(sh.ingest_stream, sh.ev_submit, 0));
-    for (int r = arena_in_place ? 1 : 0; r < nregs; r++)
-      if (regs[r].bytes)
-        CUDA_TRY(cudaMemcpyAsync(ss.d_arena + regs[r].dst_off, regs[r].root_src, regs[r].bytes, cudaMemcpyDeviceToDevice, sh.ingest_stream));
+    for (int r = arena_in_place ? 1 : 0; r < nregs; r++) {
+      const IngestRegion& g = regs[r];
+      if (g.bytes)
+        CUDA_TRY(cudaMemcpyAsync(ss.d_arena + g.dst_off, g.src, g.bytes, g.host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, sh.ingest_stream));
+    }
   }
   NCCL_TRY(nc, nc->GroupStart());
   for (Shard& sh : e->shards) {
     DeviceGuard dg(sh.device);
     ShardSlot& ss = sh.slots[si];
     int rc = 0;
-    if (arena_in_place) {
+    if (arena_in_place) {   // (device input only: regs[1] starts the descriptor arrays)
+      const size_t desc_lo = regs[1].dst_off;
       if (regs[0].bytes) {
-        void* buf = sh.gindex == 0 ? const_cast<void*>(regs[0].root_src) : (void*)ss.d_arena;   // the root sends from the caller's buffer
+        void* buf = sh.gindex == 0 ? const_cast<void*>(regs[0].src) : (void*)ss.d_arena;   // the root sends from the caller's buffer
         rc = nc->Broadcast(buf, buf, regs[0].bytes, kNcclUint8, 0, sh.comm, sh.ingest_stream);
       }
       if (!rc) rc = nc->Broadcast(ss.d_arena + desc_lo, ss.d_arena + desc_lo, all_hi - desc_lo, kNcclUint8, 0, sh.comm, sh.ingest_stream);
@@ -412,13 +375,12 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
   if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
   int rc = flush_journal(e);
   if (rc) return rc;
-  const DescLayout L(n, (uint32_t)s.bcast_index.size(), s.topics.size(), (uint32_t)s.events.size(), s.ev_topics.size());   // fits desc_cap (checked at create)
-  // Small batches ride in ONE host→device copy: the descriptor block is appended to the frame arena
-  // when it fits there (one DMA + one API call less on the latency path); otherwise two copies.
-  // Sharded engines always use the appended layout: the batch is one ingest region.
+  const DescLayout L(n, (uint32_t)s.bcast_index.size(), s.topics.size(), (uint32_t)s.events.size(), s.ev_topics.size());
+  // The descriptor block goes behind the frames in the slot's staging, so that the whole batch is one
+  // host→device copy (one ingest region on a sharded engine); it fits arena_cap (init_device).
   const size_t doff = align_up(s.arena_used, 256);
-  const bool one_copy = e->sharded || (doff + L.total <= (size_t)e->cfg.max_batch_bytes + 64 && doff + L.total <= (64u << 10));
-  uint8_t* hd = one_copy ? s.h_arena + doff : s.h_desc;
+  uint8_t* hd = s.h_arena + doff;
+  std::memset(s.h_arena + s.arena_used, 0, doff - s.arena_used);
   std::memcpy(hd + L.o_kind, s.kind.data(), n);
   std::memcpy(hd + L.o_flags, s.flags.data(), n);
   std::memcpy(hd + L.o_slot, s.slot_off16.data(), (size_t)n * 4);
@@ -433,22 +395,16 @@ int flush_open(pcdn_engine* e, uint64_t* batch_id) {
     std::memcpy(hd + L.o_etop, s.ev_topics.data(), s.ev_topics.size() * 2);
   }
   if (e->sharded) {
-    std::memset(s.h_arena + s.arena_used, 0, doff - s.arena_used);
-    if ((rc = ingest_staged(e, si, s.h_arena, doff + L.total))) return rc;
-  } else {
+    const IngestRegion staged{s.h_arena, 0, doff + L.total, true};
+    if ((rc = ingest_batch(e, si, &staged, 1, false, false))) return rc;
+  } else {   // on the main stream: a wait for the ingest stream would lengthen the latency path
     Shard& sh = e->shards[0];
     DeviceGuard dg(sh.device);
-    ShardSlot& ss = sh.slots[si];
-    if (one_copy) {
-      CUDA_TRY(cudaMemcpyAsync(ss.d_arena, s.h_arena, doff + L.total, cudaMemcpyHostToDevice, sh.stream));
-    } else {
-      CUDA_TRY(cudaMemcpyAsync(ss.d_arena, s.h_arena, align_up(s.arena_used, 16), cudaMemcpyHostToDevice, sh.stream));
-      CUDA_TRY(cudaMemcpyAsync(ss.d_desc, s.h_desc, L.total, cudaMemcpyHostToDevice, sh.stream));
-    }
+    CUDA_TRY(cudaMemcpyAsync(sh.slots[si].d_arena, s.h_arena, doff + L.total, cudaMemcpyHostToDevice, sh.stream));
   }
   for (Shard& sh : e->shards) {
     ShardSlot& ss = sh.slots[si];
-    ss.in = bind_batch(ss.d_arena, one_copy ? ss.d_arena + doff : ss.d_desc, L);
+    ss.in = bind_batch(ss.d_arena, ss.d_arena + doff, L);
   }
   s.n_msgs = n;
   rc = launch_pipeline(e, si, e->sharded);
@@ -680,18 +636,6 @@ void destroy_shard(pcdn_engine* e, Shard& sh) {
   if (sh.copy_stream) cudaStreamSynchronize(sh.copy_stream);
   if (sh.ingest_stream) cudaStreamSynchronize(sh.ingest_stream);
   if (sh.comm && e->nccl) { e->nccl->CommDestroy(sh.comm); sh.comm = nullptr; }
-  if (e->timeline && e->timeline_async && sh.ev_base) {
-    const uint32_t n = std::min(sh.tl_n, kTimelineBatches), first = sh.tl_n - n;
-    for (uint32_t j = first; j < sh.tl_n; j++) {
-      const uint32_t k = j % kTimelineBatches;
-      float t[6];
-      for (int q = 0; q < 6; q++) if (cudaEventElapsedTime(&t[q], sh.ev_base, sh.tl_ev[(size_t)k * 6 + q]) != cudaSuccess) { t[q] = -1.f; cudaGetLastError(); }
-      std::fprintf(e->timeline, "shard %u batch %llu pack_stream %d ctrl_begin %.4f direct_end %.4f match_end %.4f offsets_end %.4f pack_begin %.4f pack_end %.4f\n",
-                   sh.gindex, (unsigned long long)sh.tl_batch[k], sh.tl_ps[k], t[0], t[1], t[2], t[3], t[4], t[5]);
-    }
-    std::fflush(e->timeline);
-  }
-  for (auto& ev : sh.tl_ev) if (ev) cudaEventDestroy(ev);
   for (auto& s : sh.slots) {
     if (s.ev_done) cudaEventDestroy(s.ev_done);
     if (s.ev_ctrl) cudaEventDestroy(s.ev_ctrl);
@@ -705,7 +649,6 @@ void destroy_shard(pcdn_engine* e, Shard& sh) {
   if (sh.jstage_d) cudaFree(sh.jstage_d);
   if (sh.ev_journal) cudaEventDestroy(sh.ev_journal);
   if (sh.ev_submit) cudaEventDestroy(sh.ev_submit);
-  if (sh.ev_base) cudaEventDestroy(sh.ev_base);
   if (sh.copy_stream) cudaStreamDestroy(sh.copy_stream);
   if (sh.pack_stream) cudaStreamDestroy(sh.pack_stream);
   if (sh.ingest_stream) cudaStreamDestroy(sh.ingest_stream);
@@ -717,14 +660,11 @@ void destroy_engine(pcdn_engine* e) {
     int prev = -1;
     cudaGetDevice(&prev);
     for (Shard& sh : e->shards) destroy_shard(e, sh);
-    for (Slot& s : e->slots) {
+    for (Slot& s : e->slots)
       if (s.h_arena) cudaFreeHost(s.h_arena);
-      if (s.h_desc) cudaFreeHost(s.h_desc);
-    }
     if (prev >= 0) cudaSetDevice(prev);
     cudaGetLastError();  // a failed create must not leave its error behind for the next engine's launches
   }
-  if (e->timeline) std::fclose(e->timeline);
   delete e;
 }
 
@@ -761,12 +701,6 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
   CUDA_TRY(cudaStreamCreateWithFlags(&sh.copy_stream, cudaStreamNonBlocking));
   CUDA_TRY(cudaEventCreateWithFlags(&sh.ev_journal, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&sh.ev_submit, cudaEventDisableTiming));
-  if (e->timeline) { CUDA_TRY(cudaEventCreate(&sh.ev_base)); CUDA_TRY(cudaEventRecord(sh.ev_base, sh.stream)); }
-  if (e->timeline_async) {
-    sh.tl_ev.assign((size_t)kTimelineBatches * 6, nullptr);
-    sh.tl_batch.assign(kTimelineBatches, 0); sh.tl_ps.assign(kTimelineBatches, 0);
-    for (auto& ev : sh.tl_ev) CUDA_TRY(cudaEventCreate(&ev));
-  }
   {
     // highest priority: when a pack and the (small) control kernels of the next batch become
     // runnable together, the pack's persistent CTAs must be placed first and evenly over the SMs
@@ -822,7 +756,6 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
   sh.slots.resize(c.batch_slots);
   for (ShardSlot& s : sh.slots) {
     DEV_ALLOC(s.d_arena, e->arena_cap);
-    if (!e->sharded) DEV_ALLOC(s.d_desc, e->desc_cap);
     Work& w = s.w;
     DEV_ALLOC(w.B, (size_t)MB * Ws);
     DEV_ALLOC(w.wpre, (size_t)MB * Ws);
@@ -926,16 +859,13 @@ int init_device(pcdn_engine* e) {
   cudaGetDevice(&prev);
   const uint32_t M = c.max_batch_msgs;
   e->topics_cap = (size_t)M * 4 + 4096;
-  e->desc_cap = align_up((size_t)M * 2 + 64, 16) + (size_t)M * 20 + 64 + e->topics_cap * 2 + 64;
   // in-batch subscription events: up to max_batch_msgs of them; their topics share topics_cap
   const uint32_t max_ev = (c.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) ? M : 0;
-  e->desc_cap += (size_t)max_ev * sizeof(SubEvent) + (max_ev ? 32 : 0);
-  if (DescLayout(M, std::min(M, c.max_batch_bcast), e->topics_cap, max_ev, 0).total > e->desc_cap ||
-      (max_ev && DescLayout(M, std::min(M, c.max_batch_bcast), 1, max_ev, e->topics_cap - 1).total > e->desc_cap))
-    return fail(PCDN_EINVAL, "the descriptor block of a full batch exceeds desc_cap");
-  // sharded engines keep frames + descriptor block in one ingest region (and device-input batches
-  // need room for the descriptor arrays behind the frames)
-  e->arena_cap = c.max_batch_bytes + 64 + (e->sharded ? 256 + e->desc_cap : 0);
+  // The largest descriptor block: DescLayout grows with every count, so a full batch bounds every batch.
+  // Splitting the topic entries between messages and events adds at most 16 bytes of alignment.
+  const size_t desc_cap = DescLayout(M, std::min(M, c.max_batch_bcast), e->topics_cap, max_ev, 0).total + (max_ev ? 16 : 0);
+  e->frames_cap = c.max_batch_bytes + 64;
+  e->arena_cap = e->frames_cap + 256 + desc_cap;
   e->has_device = true;
   for (size_t i = 0; i < e->shards.size(); i++) {
     int rc = init_shard(e, e->shards[i], ndev, i == 0 ? c.stream : nullptr);
@@ -945,7 +875,6 @@ int init_device(pcdn_engine* e) {
   for (Slot& s : e->slots) {
     int rc = pin_alloc(&s.h_arena, e->arena_cap);
     if (rc) return rc;
-    if (!e->sharded && (rc = pin_alloc(&s.h_desc, e->desc_cap))) return rc;
   }
   if (e->sharded && e->ingest == PCDN_INGEST_NCCL) {
     int rc = init_nccl(e);
@@ -1018,12 +947,6 @@ int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
         if (cfg->devices[i] == cfg->devices[j])
           return fail(PCDN_EINVAL, "PCDN_INGEST_NCCL needs one GPU per shard (use PCDN_INGEST_HOST for shards that share a device)");
   pcdn_engine* e = new pcdn_engine();
-  if (const char* tl = std::getenv("PCDN_TIMELINE")) {
-    e->timeline = std::fopen(tl, "a");
-    e->timing = e->timeline != nullptr;
-    const char* as = std::getenv("PCDN_TIMELINE_ASYNC");
-    e->timeline_async = e->timeline && as && as[0] == '1';
-  }
   e->cfg = *cfg;
   e->identity = cfg->identity ? cfg->identity : "/";
   e->cfg.identity = e->identity.c_str();
@@ -1580,7 +1503,7 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
     return fail(PCDN_EINVAL, "device batch exceeds configured capacities");
   const uint32_t n = b->n_msgs, nb = b->n_bcast;
   const bool shared = (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) != 0;
-  if (shared && b->arena_bytes > e->arena_cap)
+  if (shared && b->arena_bytes > e->frames_cap)
     return fail(PCDN_ENOSPC, "device batch frames exceed the pinned payload staging (max_batch_bytes)");
   // sharded engines: the frames at the start of a receiving shard's arena, the descriptor block behind them
   const DescLayout L(n, nb, b->n_topics_total);
@@ -1612,7 +1535,7 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
         {b->slot_off16, doff + L.o_slot, (size_t)n * 4}, {b->raw_len, doff + L.o_len, (size_t)n * 4},
         {b->aux_off, doff + L.o_aoff, (size_t)n * 4}, {b->aux_len, doff + L.o_alen, (size_t)n * 4},
         {b->bcast_index, doff + L.o_bidx, (size_t)nb * 4}, {b->topics, doff + L.o_top, (size_t)b->n_topics_total * 2}};
-    if ((rc = ingest_device(e, si, regs, 9, arena_in_place, !ready))) { abandon_open(e); return rc; }
+    if ((rc = ingest_batch(e, si, regs, 9, arena_in_place, !ready))) { abandon_open(e); return rc; }
   }
   for (Shard& sh : e->shards) {
     ShardSlot& ss = sh.slots[si];
@@ -1907,14 +1830,6 @@ int pcdn_release_batch(pcdn_engine* e, uint64_t batch_id) {
     const bool payload_copy = s.device_input && (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD);
     if (!ss.polled && (!s.device_input || payload_copy))
       CUDA_TRY(cudaEventSynchronize((e->sharded && !payload_copy) ? ss.ev_ingest : ss.ev_done));
-    if (e->timeline && ss.timed && !e->timeline_async) {   // diagnostic: where this batch's stages ran on the shard's clock (blocks until the pack is done)
-      CUDA_TRY(cudaEventSynchronize(ss.ev_done));
-      float t[6];
-      for (int k = 0; k < 6; k++) if (cudaEventElapsedTime(&t[k], sh.ev_base, ss.ev[k]) != cudaSuccess) { t[k] = -1.f; cudaGetLastError(); }
-      std::fprintf(e->timeline, "shard %u batch %llu pack_stream %d ctrl_begin %.4f direct_end %.4f match_end %.4f offsets_end %.4f pack_begin %.4f pack_end %.4f\n",
-                   sh.gindex, (unsigned long long)batch_id, (int)ss.on_pack_stream, t[0], t[1], t[2], t[3], t[4], t[5]);
-      std::fflush(e->timeline);
-    }
     // ring space may be reused only after the pack that filled it has finished
     CUDA_TRY(cudaStreamWaitEvent(sh.stream, ss.ev_done, 0));
     launch_release(sh.dev, ss.w.batch_units, ss.w.stats, sh.stream);
@@ -1993,7 +1908,7 @@ int pcdn_get_stats(pcdn_engine* e, pcdn_stats* out) {
 }
 int pcdn_set_timing(pcdn_engine* e, int on) {
   LOCK;
-  e->timing = on != 0 || e->timeline != nullptr;
+  e->timing = on != 0;
   return 0;
 }
 int pcdn_ring_info(pcdn_engine* e, void** dev_base, uint64_t* ring_bytes, uint32_t* max_conns) {

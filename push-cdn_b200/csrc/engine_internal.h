@@ -76,8 +76,7 @@ constexpr uint32_t kDirectPublishMaxConns = 65536;  // = kSmallCtrlConns: the sh
 // One shard's share of a batch slot: the batch as it lies in that GPU's memory, the kernels' scratch
 // and the result buffers the host reads.
 struct ShardSlot {
-  uint8_t* d_arena = nullptr;   // frames (sharded engines: frames + descriptor block, one ingest region)
-  uint8_t* d_desc = nullptr;    // descriptor block (single-shard two-copy path)
+  uint8_t* d_arena = nullptr;   // frames, and the descriptor block behind them (one ingest region)
   Work w{};
   BatchIn in{};
   // results
@@ -98,8 +97,7 @@ struct ShardSlot {
   cudaEvent_t ev_early = nullptr;  // early counters are in h_early (copy stream)
   cudaEvent_t ev_ingest = nullptr; // the batch has arrived in d_arena (ingest stream)
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  bool on_pack_stream = false;     // this batch's pack was launched on the pack stream
-  bool timed = false;
+  bool timed = false;              // the stage events ev[] were recorded for this batch (pcdn_set_timing)
   bool polled = false;             // results of this shard have been fetched
 };
 
@@ -125,9 +123,6 @@ struct Shard {
   int nccl_ranks = 0;
   int prev_slot[2] = {-1, -1};      // the two most recently launched slots (newest first)
   bool fat_only = false;            // the last completed batch packed message-major tiles only (no connection-major message)
-  cudaEvent_t ev_base = nullptr;    // PCDN_TIMELINE: time zero of this shard's timeline dump
-  std::vector<cudaEvent_t> tl_ev;   // PCDN_TIMELINE_ASYNC: 6 stage events for each of the last kTimelineBatches launches
-  std::vector<uint64_t> tl_batch; std::vector<int> tl_ps; uint32_t tl_n = 0;
   cudaEvent_t ev_submit = nullptr;  // device-input batches: "everything queued on the main stream so far"
   std::vector<void*> dev_allocs, pin_allocs;
 };
@@ -138,7 +133,7 @@ struct Slot {
   uint64_t batch_id = 0;
   bool device_input = false;
   // host staging while open
-  uint8_t* h_arena = nullptr;   // pinned
+  uint8_t* h_arena = nullptr;   // pinned: frames, and the descriptor block behind them once the batch is flushed
   size_t arena_used = 0;
   std::vector<uint8_t> kind, flags;
   std::vector<uint32_t> slot_off16, raw_len, aux_off, aux_len, bcast_index;
@@ -150,7 +145,6 @@ struct Slot {
   uint64_t ingress_bytes = 0;   // pool permits held by this batch
   std::chrono::steady_clock::time_point t_launch;
   bool devparse = false;        // some messages carry MSGF_DEVPARSE (k_parse runs first)
-  uint8_t* h_desc = nullptr;    // pinned descriptor block
   bool counted = false;         // counters of this batch have been added to the engine stats
   // merged view of a sharded batch for pcdn_poll (host copy of the shards' span tables)
   std::vector<pcdn_span> merged_spans;
@@ -189,12 +183,12 @@ struct pcdn_engine {
   int open_slot = -1;
   uint64_t next_batch_id = 1;
   std::vector<uint64_t> inflight;  // submit order
-  size_t desc_cap = 0, topics_cap = 0, arena_cap = 0;
+  size_t topics_cap = 0;
+  size_t frames_cap = 0;          // frame bytes a slot's staging holds (bounds a shared-payload device batch's arena_bytes)
+  size_t arena_cap = 0;           // a slot's staging / ingest region: frames_cap, 256-byte alignment, the largest descriptor block
   uint64_t pool_bytes = 0;        // PCDN_FLAG_OUTPUT_POOL: bytes of the output pool per shard
   std::vector<UpdSlot> h_slot; std::vector<uint32_t> h_kslot; std::vector<uint8_t> h_kbytes;  // journal parts common to all shards
   bool timing = false;
-  bool timeline_async = false;      // PCDN_TIMELINE_ASYNC=1: never block; the timeline is written when the engine is destroyed
-  FILE* timeline = nullptr;         // PCDN_TIMELINE=<file>: per-batch device timestamps of the stage events (diagnostic)
   pcdn_message_hook hook[2] = {nullptr, nullptr};  // [origin]: MessageHookDef of user / broker connections
   void* hook_user[2] = {nullptr, nullptr};
   uint64_t inflight_bytes = 0;  // Limiter analogue: accepted frame bytes whose batch is not released yet

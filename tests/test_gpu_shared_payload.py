@@ -298,7 +298,8 @@ def test_sharded_device_resident_batch_shared(pcdn):
 @pytest.mark.parametrize("ready", [False, True])
 def test_device_resident_batch_payload(pcdn, ready):
     """pcdn_submit_device on one GPU: the frames are copied once into pinned staging, batch_payload
-    returns them, and the streams match the oracle; an arena larger than the staging is ENOSPC"""
+    returns them, and the streams match the oracle; an arena of max_batch_bytes + 64 bytes fits the
+    staging, a larger one is ENOSPC"""
     import torch
 
     w = World(SharedPcdn(pcdn), max_conns=2048, max_batch_bytes=1 << 20)
@@ -358,12 +359,31 @@ def test_device_resident_batch_payload(pcdn, ready):
         got = w.e.collect_frames(res)
         w.e.release_batch(b)
         assert got == w.expect()
-    big = pcdn.DeviceBatch(M, len(bidx), d_arena.data_ptr(), (1 << 20) + 4096, d_kind.data_ptr(), d_flags.data_ptr(), d_slot.data_ptr(),
-                           d_len.data_ptr(), d_aoff.data_ptr(), d_alen.data_ptr(), d_topics.data_ptr(), len(topics), d_bidx.data_ptr())
-    with pytest.raises(pcdn.PcdnError) as ei:
-        w.e.submit_device(big)
-    assert ei.value.code == -5                          # PCDN_ENOSPC, nothing launched
-    assert w.e.next_batch() == 0
+    # the staging holds max_batch_bytes + 64 frame bytes: an arena of exactly that size is staged whole
+    cap = (1 << 20) + 64
+    d_full = torch.zeros(cap + 16, dtype=torch.uint8, device=dev)
+    d_full[:len(arena)] = d_arena[:len(arena)]
+    torch.cuda.synchronize(dev)
+
+    def sized(ptr, arena_bytes):
+        s = pcdn.DeviceBatch(M, len(bidx), ptr, arena_bytes, d_kind.data_ptr(), d_flags.data_ptr(), d_slot.data_ptr(),
+                             d_len.data_ptr(), d_aoff.data_ptr(), d_alen.data_ptr(), d_topics.data_ptr(), len(topics), d_bidx.data_ptr())
+        s.hints = db.hints
+        return s
+
+    oracle_batch()
+    b = w.e.submit_device(sized(d_full.data_ptr(), cap))
+    res = w.e.poll(b)
+    assert res.status == 0
+    assert C.string_at(w.e.batch_payload(b), cap) == bytes(arena) + bytes(cap - len(arena))
+    got = w.e.collect_frames(res)
+    w.e.release_batch(b)
+    assert got == w.expect()
+    for arena_bytes in (cap + 16, (1 << 20) + 4096):
+        with pytest.raises(pcdn.PcdnError) as ei:
+            w.e.submit_device(sized(d_full.data_ptr(), arena_bytes))
+        assert ei.value.code == -5                      # PCDN_ENOSPC, nothing launched
+        assert w.e.next_batch() == 0
     w.e.close()
 
 
