@@ -228,11 +228,14 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   s.w.spans = s.spans_mapped ? s.d_spans_map : s.d_spans_dev;
   s.w.overflow = s.spans_mapped ? s.d_ovf_map : s.d_ovf_dev;
   const bool zero_in_kernel = fused && !devparse && !retry;  // (k_parse counts into the batch counters before the fused kernel)
+  // regular pipeline: k_match zeroes the counters when it is the batch's first kernel (the direct lookup
+  // counts into them from many CTAs, and k_parse before it: those batches keep the memset)
+  const bool zero_in_match = !fused && !devparse && !retry && !has_direct && s.in.n_bcast > 0;
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[0], st));
   if (retry) {
     launch_pool_retry_begin(sh.dev, s.w, st);
   } else {
-    if (!zero_in_kernel) launch_batch_begin(sh.dev, s.w, s.in, has_direct, st);
+    if (!zero_in_kernel && !zero_in_match) launch_batch_begin(sh.dev, s.w, s.in, has_direct, st);
     if (devparse) launch_parse(sh.dev, s.w, s.in, st);
     if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
   }
@@ -241,7 +244,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
     launch_ctrl_small(sh.dev, s.w, s.in, has_direct, zero_in_kernel, s.d_stats_pub, retry, st);
     if (s.timed) { CUDA_TRY(cudaEventRecord(s.ev[2], st)); CUDA_TRY(cudaEventRecord(s.ev[3], st)); }
   } else {
-    if (!retry) launch_match(sh.dev, s.w, s.in, st);
+    if (!retry) launch_match(sh.dev, s.w, s.in, zero_in_match ? s.w.stats : nullptr, st);
     if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[2], st));
     if (!retry) launch_plan(sh.dev, s.w, s.in, st);
     launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);   // pool mode: a pure function of the scratch
@@ -264,10 +267,12 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   // +2 % with 3)
   uint32_t pack_variant = e->cfg.pack_variant;
   if (!((pack_variant >> 8) & 15u)) pack_variant |= (fat_overlap ? 3u : 4u) << 8;
-  launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, ps);
+  // the final counters reach h_stats from the last pack kernel (mapped memory, covered by ev_done); only a
+  // batch without a pack launch copies them
+  const bool published = launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, fused ? nullptr : s.d_stats_pub, ps);
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[5], ps));
   CUDA_TRY(cudaGetLastError());
-  if (!fused) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));
+  if (!fused && !published) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));
   CUDA_TRY(cudaEventRecord(s.ev_done, ps));
   return 0;
 }
@@ -775,6 +780,10 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
     DEV_ALLOC(w.jidx, M);
     DEV_ALLOC(w.efat, cap_fat);
     DEV_ALLOC(w.ecm, cap_fat);
+    // A connection-major message has at least N/16 recipients (kCmDenseShift), and a batch past cap_fat
+    // fat + cm deliveries is refused before k_offsets, so n_cm <= 16 * cap_fat / N and the run starts
+    // need groups * N <= (n_cm / 8 + 1) * N <= 2 * cap_fat + N entries (and never more than MB / 8 groups).
+    DEV_ALLOC(w.cmrun, std::min<size_t>(((size_t)MB + kCmGroup - 1) / kCmGroup * Ns, 2 * cap_fat + Ns));
     DEV_ALLOC(w.ethin, cap_thin);
     w.cap_fat = (uint32_t)std::min<size_t>(cap_fat, 0xFFFFFFFFu);
     w.cap_thin = (uint32_t)std::min<size_t>(cap_thin, 0xFFFFFFFFu);
@@ -814,8 +823,7 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
     DEV_ALLOC(w.msg_status, M);
     PIN_ALLOC(s.h_msg_status, M);
     DEV_ALLOC(w.stats, 1);
-    if (sh.direct_publish) PIN_ALLOC_MAPPED(s.h_stats, s.d_stats_pub, 1);
-    else PIN_ALLOC(s.h_stats, 1);
+    PIN_ALLOC_MAPPED(s.h_stats, s.d_stats_pub, 1);   // written by the kernel that ends the batch
     PIN_ALLOC(s.h_early, 1);
     CUDA_TRY(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
     CUDA_TRY(cudaEventCreateWithFlags(&s.ev_ctrl, cudaEventDisableTiming));

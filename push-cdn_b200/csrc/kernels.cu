@@ -458,7 +458,10 @@ __device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn&
 // loads of the bitmap rows, no block-level synchronisation: the popcount prefix of a 256-word block
 // is a lane-local prefix plus one warp scan).  grid = (ceil(nblk / 8), n_bcast).
 template <bool EVENTS>
-__global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w) {
+__global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, BatchStats* zero) {
+  // the batch's first kernel when it has no direct message and no device parse: it zeroes the counters
+  // (nothing else in this launch touches them) instead of a memset on the stream
+  if (zero && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x < sizeof(BatchStats) / 4) reinterpret_cast<uint32_t*>(zero)[threadIdx.x] = 0;
   const uint32_t j = blockIdx.y, lane = lane_id();
   const uint32_t blk = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (blk >= s.nblk) return;  // warp-uniform
@@ -524,13 +527,13 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w) {
     if (lane == 0) { w.D[m] = carry; w.jidx[m] = j; w.done[j] = 0; }
   }
 }
-void launch_match(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st) {
+void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, cudaStream_t st) {
   if (!b.n_bcast) return;
   dim3 grid((s.nblk + 7) / 8, b.n_bcast);
   // (a batch with in-batch subscription events takes its own instantiation: the one without them keeps
   //  the registers and occupancy it has without the patch)
-  if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true><<<grid, 256, 0, st>>>(s, b, w);
-  else PCDN_COUNT_LAUNCH, k_match<false><<<grid, 256, 0, st>>>(s, b, w);
+  if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true><<<grid, 256, 0, st>>>(s, b, w, zero);
+  else PCDN_COUNT_LAUNCH, k_match<false><<<grid, 256, 0, st>>>(s, b, w, zero);
 }
 
 // =============================================================================== K1p plan
@@ -781,10 +784,23 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
     w.edir[m] = make_uint2(c, off);
   };
 
+  // Connection-major records: one cmrun word per (group, connection) instead of one ecm entry per
+  // record when the connection's records of the group are one run, which is what the pack merges
+  // into one bulk store anyway.  Per thread: cm_last = cm rank of its last connection-major record
+  // (kOffInvalid: none yet), cm_start = that group's run start or kCmBroken | position, cm_first = the
+  // ecm index of the group's first record, cm_next = the unit after the run.  (In shared memory, and
+  // the cmrun row found through a pointer staged per message: kept in registers, or indexed with 64-bit
+  // arithmetic here, they cost k_offsets<false> 8 more registers and with them 2 of its 8 CTAs per SM.)
+  __shared__ uint32_t cm_last_[NT], cm_first_[NT], cm_start_[NT], cm_next_[NT];
+  uint32_t& cm_start = cm_start_[threadIdx.x];
+  uint32_t& cm_next = cm_next_[threadIdx.x];
+  cm_last_[threadIdx.x] = kOffInvalid;
+
   // Broadcasts are taken 32 at a time: the block stages their per-message metadata in shared
   // memory once, and every warp fetches its 32 match words / rank prefixes with ONE load per lane
   // (lane i ↔ message j0+i) instead of a dependent chain of warp-uniform loads per message.
-  __shared__ uint32_t m_mb[32], m_len[32], m_eb[32], m_slot[32], m_cls[32];
+  __shared__ uint32_t m_mb[32], m_len[32], m_eb[32], m_slot[32], m_cls[32], m_cmr[32];
+  __shared__ uint32_t* m_run[32];   // the cmrun row of the message's group (connection-major messages)
   for (uint32_t j0 = 0; j0 < b.n_bcast; j0 += 32) {
     const uint32_t nj = min(32u, b.n_bcast - j0);
     __syncthreads();
@@ -794,6 +810,11 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
       m_mb[threadIdx.x] = m;
       m_len[threadIdx.x] = b.raw_len[m];
       m_cls[threadIdx.x] = cl;
+      if (cl == CLS_CM) {
+        const uint32_t r = w.cm_rank[m];
+        m_cmr[threadIdx.x] = r;
+        m_run[threadIdx.x] = w.cmrun + (size_t)(r / kCmGroup) * s.N;
+      }
       m_eb[threadIdx.x] = cl != CLS_THIN ? w.eb_fat[m] : w.eb_thin[m];
       m_slot[threadIdx.x] = b.slot_off16[m];
     }
@@ -813,10 +834,29 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
       if (HAS_DIRECT) while (dp < de && dmsg[dp] < mb) { emit_direct(dmsg[dp]); dp++; }  // keep batch order (R9)
       if ((word >> lane) & 1u) {
         const uint32_t rank = p + __popc(word & lt), len = m_len[i];
-        const uint32_t off = alloc_record(k, rec_units(s, len), R, len);
+        const uint32_t u = rec_units(s, len);
+        const uint32_t off = alloc_record(k, u, R, len);
         const uint32_t cl = m_cls[i];
-        if (cl == CLS_CM) w.ecm[m_eb[i] + rank] = off;
-        else if (cl == CLS_FAT) w.efat[m_eb[i] + rank] = make_uint2(c, off);
+        if (cl == CLS_CM) {
+          // The group stops being one run at the first record that does not follow the previous one (a
+          // wrap, another record of this connection in between, an overflow): from there on its records
+          // get ecm entries, and so does the first one (the run start); the pack follows the run up to
+          // that position.
+          uint32_t* row = m_run[i];
+          const uint32_t r = m_cmr[i];
+          if ((r ^ cm_last_[threadIdx.x]) >= kCmGroup) {   // first record of a group (cm ranks ascend with the batch order)
+            cm_start = off != kOffInvalid ? off : kCmBroken | (r & (kCmGroup - 1));
+            cm_first_[threadIdx.x] = m_eb[i] + rank;
+            row[c] = cm_start;
+          } else if (cm_start < kCmBroken && off != cm_next) {
+            w.ecm[cm_first_[threadIdx.x]] = cm_start;
+            cm_start = kCmBroken | (r & (kCmGroup - 1));
+            row[c] = cm_start;
+          }
+          if (cm_start >= kCmBroken) w.ecm[m_eb[i] + rank] = off;
+          cm_last_[threadIdx.x] = r;
+          cm_next = off + u;
+        } else if (cl == CLS_FAT) w.efat[m_eb[i] + rank] = make_uint2(c, off);
         else w.ethin[m_eb[i] + rank] = make_uint4(c, off, m_slot[i], len);
       }
     }
@@ -1098,7 +1138,7 @@ __global__ void k_pool_retry_begin(BatchStats* bs) {
   bs->status = 0;
   bs->n_deliveries = 0; bs->bytes_out = 0;
   bs->n_spans = 0; bs->n_runs = 0; bs->n_overflow = 0;
-  bs->tile_cursor = 0; bs->cm_cursor = 0;
+  bs->tile_cursor = 0; bs->cm_cursor = 0; bs->ctas_done = 0;
 }
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st) {
   cudaMemsetAsync(w.lb_state, 0, ((size_t)s.N / 256 + 1) * 8, st);
@@ -1222,7 +1262,7 @@ __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& 
     }
     __syncthreads();
     if (t_info[0] >= ntiles) break;
-    const uint32_t gcount = t_info[2];
+    const uint32_t grp = t_info[1], gcount = t_info[2];
     if (t_info[3]) {
       // New group: shared memory is re-staged.  Bulk stores issued for earlier tiles only have to
       // be drained HERE (they read the old frames) — not after every tile, so the TMA store
@@ -1258,17 +1298,31 @@ __device__ __forceinline__ void pack_cm_phase(const DevState& s, const BatchIn& 
       const uint32_t myword = lane < gcount ? w.B[(size_t)g_j[lane] * s.W + wd] : 0u;
       const uint32_t any = __reduce_or_sync(0xffffffffu, myword);
       if (!any) continue;
-      // ring offset of (connection = wd*32+lane, message i of the group), or invalid
+      uint32_t mine = 0;  // bit i: connection wd*32+lane receives message i of the group
+#pragma unroll
+      for (int i = 0; i < (int)kCmGroup; i++)
+        mine |= ((__shfl_sync(0xffffffffu, myword, i) >> lane) & 1u) << i;
+      mine &= (1u << gcount) - 1u;
+      // ring offset of (connection = wd*32+lane, message i of the group), or invalid: from the run start
+      // (k_offsets' cmrun) while the connection's records of the group follow each other, from the scatter
+      // list for its first record and from the position where they stop following each other
       uint32_t offs[kCmGroup];
+      const uint32_t run = mine ? w.cmrun[(size_t)grp * s.N + wd * 32 + lane] : kOffInvalid;
+      const uint32_t brk = run >= kCmBroken ? run - kCmBroken : kCmGroup;
+      uint32_t cur = run;
+      bool first = true;
 #pragma unroll
       for (int i = 0; i < (int)kCmGroup; i++) {
-        const uint32_t wordi = __shfl_sync(0xffffffffu, myword, i);
         offs[i] = kOffInvalid;
-        if ((uint32_t)i < gcount && ((wordi >> lane) & 1u)) {
-          const uint32_t j = g_j[i];
-          const uint32_t idx = g_eb[i] + w.base[(size_t)j * s.nblk + wd / kBlockWords] + w.wpre[(size_t)j * s.W + wd] +
-                               __popc(wordi & ((1u << lane) - 1u));
-          offs[i] = w.ecm[idx];
+        if ((mine >> i) & 1u) {
+          if (brk < kCmGroup && (first || (uint32_t)i >= brk)) {   // (rare: lanes of one warp may get here apart, so the match word is re-read)
+            const uint32_t j = g_j[i];
+            const size_t at = (size_t)j * s.W + wd;
+            cur = w.ecm[g_eb[i] + w.base[(size_t)j * s.nblk + wd / kBlockWords] + w.wpre[at] + __popc(w.B[at] & ((1u << lane) - 1u))];
+          }
+          offs[i] = cur;
+          first = false;
+          if (cur != kOffInvalid) cur += g_units[i];
         }
       }
       // one lane = one connection: merge adjacent records into runs, one bulk store per run
@@ -1351,32 +1405,53 @@ __device__ __forceinline__ void pack_direct_phase(const DevState& s, const Batch
   }
 }
 
+// The kernel that ends a batch publishes its final counters into mapped host memory, so that the batch's
+// ev_done covers them without a device-to-host copy on the stream between one pack and the next batch.
+// Every CTA counts itself done (also when the batch was refused); the last one copies the counters.
+__device__ __forceinline__ void publish_if_last(const Work& w, BatchStats* publish) {
+  if (!publish) return;
+  __shared__ uint32_t last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = atomicAdd(&w.stats->ctas_done, 1u) == gridDim.x - 1 ? 1u : 0u;
+  }
+  __syncthreads();
+  if (last && threadIdx.x < sizeof(BatchStats) / 4) {
+    __threadfence();
+    reinterpret_cast<volatile uint32_t*>(publish)[threadIdx.x] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + threadIdx.x);
+    __threadfence_system();
+  }
+}
+
 // One launch runs the pack phases back to back in persistent CTAs (each phase pulls its own
 // work from its own cursor, so CTAs drift from phase to phase without a grid barrier; the phases
 // write disjoint records).
-__global__ void __launch_bounds__(256) k_pack(DevState s, BatchIn b, Work w, int do_direct) {
+__global__ void __launch_bounds__(256) k_pack(DevState s, BatchIn b, Work w, int do_direct, BatchStats* publish) {
   __shared__ __align__(128) uint8_t buf[kCmGroup * kCmMaxBytes];  // 32 KB; the fat phase uses the first 16 KB
   __shared__ __align__(8) uint64_t bars[2];
-  if (w.stats->status) return;
-  if (threadIdx.x == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (!w.stats->status) {
+    if (threadIdx.x == 0) {
+      mbar_init(&bars[0], 1);
+      mbar_init(&bars[1], 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    pack_cm_phase(s, b, w, buf, &bars[0]);
+    __syncthreads();
+    pack_fat_phase(s, b, w, buf, &bars[1]);
+    pack_thin_phase(s, b, w);
+    if (do_direct) pack_direct_phase(s, b, w);
   }
-  __syncthreads();
-  pack_cm_phase(s, b, w, buf, &bars[0]);
-  __syncthreads();
-  pack_fat_phase(s, b, w, buf, &bars[1]);
-  pack_thin_phase(s, b, w);
-  if (do_direct) pack_direct_phase(s, b, w);
+  publish_if_last(w, publish);
 }
 // Batches dominated by direct messages run the direct phase as its own launch at full occupancy
 // (no shared memory, 8 CTAs per SM): a warp per record is a chain of two dependent DRAM reads
 // (list entry, frame) before its stores, so the phase scales with warps in flight — 24 → 48
 // warps per SM is faster on the 1 M x 512 B direct workload (config C4).
-__global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, Work w) {
-  if (w.stats->status) return;
-  pack_direct_phase(s, b, w);
+__global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, Work w, BatchStats* publish) {
+  if (!w.stats->status) pack_direct_phase(s, b, w);
+  publish_if_last(w, publish);
 }
 
 // =============================================================================== K2r pack (reference records)
@@ -1393,8 +1468,8 @@ __device__ __forceinline__ void st_ref_record(uint8_t* dst, uint32_t raw_len, ui
 // is found by a binary search of eb_fat), thin (ethin carries everything) and direct (edir, entry m =
 // message m).  Entries of one message are in connection order, so a warp's 32 stores go to 32
 // consecutive connections; a connection's records of successive messages are adjacent in its ring.
-__global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w, int do_direct) {
-  if (w.stats->status) return;
+__global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w, int do_direct, BatchStats* publish) {
+  if (w.stats->status) { publish_if_last(w, publish); return; }
   const uint32_t nfat = w.stats->n_fat_entries, nthin = w.stats->n_thin_entries;
   const uint64_t nft = (uint64_t)nfat + nthin, total = nft + (do_direct ? b.n_msgs : 0u);
   const uint32_t pool_base = w.stats->pool_base;
@@ -1421,25 +1496,29 @@ __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w,
     if (!thin) { slot = b.slot_off16[m]; len = b.raw_len[m]; }
     st_ref_record(conn_out(s, w, conn, pool_base) + (size_t)off * kUnit, len, slot, bid);
   }
+  publish_if_last(w, publish);
 }
 
 // pack_variant (pcdn_config) holds launch geometry only: bits 8-11 = CTAs per SM of k_pack (the engine
 // fills in its default, launch_shard_pipeline; 3 if none), bits 12-15 = CTAs per SM of the separate
 // direct pack (default 8 = full occupancy).  Neither changes what is written, only how the persistent
 // CTAs share the work.
-void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms, cudaStream_t st) {
+bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
+                 BatchStats* publish, cudaStream_t st) {
   if (s.shared_payload) {   // (the CTA counts of pack_variant describe k_pack and k_pack_direct: they do not apply here)
-    if (b.n_bcast || n_direct) PCDN_COUNT_LAUNCH, k_pack_ref<<<(uint32_t)n_sms * 8, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0);
-    return;
+    if (!b.n_bcast && !n_direct) return false;
+    PCDN_COUNT_LAUNCH, k_pack_ref<<<(uint32_t)n_sms * 8, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
+    return true;
   }
   const bool direct_separate = n_direct >= kThinSeparateMin;
   const uint32_t ctas_per_sm = ((pack_variant >> 8) & 15u) ? ((pack_variant >> 8) & 15u) : 3;
   const uint32_t grid = (uint32_t)n_sms * ctas_per_sm;
   const int do_direct = (n_direct && !direct_separate) ? 1 : 0;
   if (b.n_bcast || do_direct)  // (a batch of nothing but many direct messages has no work for this kernel)
-    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct);
+    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct, direct_separate ? nullptr : publish);
   const uint32_t dctas = ((pack_variant >> 12) & 15u) ? ((pack_variant >> 12) & 15u) : 8u;
-  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w);
+  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w, publish);
+  return direct_separate || b.n_bcast || do_direct;
 }
 
 // =============================================================================== release

@@ -35,6 +35,9 @@ namespace pcdn {
 
 constexpr uint32_t kUnit = 32;               // record alignment in ring (bytes) = PCDN_RECORD_ALIGN
 constexpr uint32_t kOffInvalid = 0xFFFFFFFFu;
+// Work::cmrun: kCmBroken | p = the (group, connection) pair is one run up to group position p only.  Never a
+// unit offset: a ring holds at most 2 GiB = 2^26 units, a connection's pool region less than 2^31.
+constexpr uint32_t kCmBroken = 0xFFFFFFF0u;
 constexpr uint32_t kConnNone = 0xFFFFFFFFu;
 constexpr uint32_t kFatMin = 32;             // >= this many recipients → staged (fat) path
 constexpr uint32_t kChunkBytes = 16384;      // shared-memory staging chunk of the fat path
@@ -147,7 +150,7 @@ struct BatchStats {
   uint32_t pool_base;       // pool mode: first unit of this batch's region (span offsets are relative to it)
   uint32_t pool_units;      // pool mode: units of the region
   uint32_t pool_skip;       // pool mode: units skipped at the end of the pool to keep the region contiguous
-  uint32_t reserved;
+  uint32_t ctas_done;       // CTAs of the kernel that ends the batch that have finished (the last one publishes)
 };
 
 // ring buffer of batch regions inside the output pool (units of 32 B); batches are released in order
@@ -180,7 +183,14 @@ struct Work {
   uint32_t* jidx;        // [max_msgs] message index → broadcast slot j
   uint2* efat;           // [cap_fat]  {conn, ring offset in units} — message-major (fat) class
   uint32_t* ecm;         // [cap_fat]  ring offset in units — connection-major class (the connection is
-                         //            implied by the rank, so 4 bytes per delivery instead of 8)
+                         //            implied by the rank, so 4 bytes per delivery instead of 8); written only
+                         //            where cmrun says so
+  uint32_t* cmrun;       // [min(MB/8 groups * N, 2 * cap_fat + N)] at g * N + c: the first unit of connection c's
+                         //            records of connection-major group g (kCmGroup messages in cm rank order) when
+                         //            they are ONE contiguous run in group order; kCmBroken | p when they are one
+                         //            run only up to group position p (a wrap, another record of c in between, an
+                         //            overflow): ecm then holds the first record's offset and those from p on.
+                         //            Unset when c matches nothing of the group.
   uint4* ethin;          // [cap_thin] {conn, ring offset in units, slot_off16, raw_len}
   uint32_t cap_fat, cap_thin;
   // Direct hits grouped by target connection WITHOUT a sort: the lookup counts hits per connection
@@ -228,7 +238,8 @@ void launch_apply_updates(const DevState& s, const Upd32* u32, uint32_t n32, con
 void launch_batch_begin(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, cudaStream_t st);
 void launch_parse(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st);
-void launch_match(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
+// zero: the batch's counters, zeroed by k_match before any kernel writes one (null: zeroed earlier)
+void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, cudaStream_t st);
 void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st);
 // fused match + plan + offsets for N <= kSmallCtrlConns and n_msgs <= kSmallCtrlMsgs (one cluster launch)
@@ -236,7 +247,10 @@ void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool 
                        BatchStats* publish, bool offsets_only, cudaStream_t st);
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);
-void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms, cudaStream_t st);
+// publish (mapped host memory): the last pack kernel copies the batch's final counters there; returns false when
+// the batch launches no pack kernel, so nothing was published
+bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
+                 BatchStats* publish, cudaStream_t st);
 void launch_release(const DevState& s, const uint32_t* batch_units, const BatchStats* stats, cudaStream_t st);
 void launch_pool_init(const DevState& s, cudaStream_t st);
 unsigned long long kernel_launches();   // launches issued by this library in this process so far
