@@ -81,7 +81,8 @@ enum { PCDN_TO_USERS_ONLY = 1 };
 #define PCDN_RECORD_ALIGN 32u
 
 typedef struct pcdn_config {
-  uint32_t struct_size;         /* = sizeof(pcdn_config); ABI guard                             */
+  uint32_t struct_size;         /* = sizeof(pcdn_config); ABI guard.  offsetof(pcdn_config, ref_min_bytes)
+                                 * (the size before that field was added) is accepted as ref_min_bytes = 0 */
   int32_t device;               /* CUDA ordinal; < 0 = host-only state mirror (no data path)    */
   uint32_t max_conns;           /* capacity of the dense connection-id space (users + brokers)  */
   uint32_t max_topics;          /* rows of the subscription bitmap; 256 = wire-exact (Topic=u8) */
@@ -127,6 +128,20 @@ typedef struct pcdn_config {
                                  * that may be in flight (accepted, their batch not yet released); 0 = unlimited.
                                  * The reference awaits the semaphore; here a frame that does not fit is refused
                                  * with PCDN_EAGAIN and the caller retries after releasing a batch. */
+  /* Delivery by reference above a size threshold: a routed message (broadcast or direct) whose raw length is
+   * >= ref_min_bytes is delivered as ONE reference record per recipient (the layout of
+   * PCDN_FLAG_SHARED_PAYLOAD below, its payload resolved through pcdn_batch_payload); every shorter message
+   * keeps its framed copy, the wire bytes a consumer can send straight from the rings.  A message is
+   * delivered one way or the other, never both, and a connection's span may hold both kinds of record, in
+   * batch order.  Spans, runs, n_records, bytes_out (4 + L per delivery), pool_base, wrap, release and retry
+   * keep their meaning.  0 = off (every delivery a framed copy).  The threshold decides which deliveries
+   * need the host payload, so it is the host's to choose; pcdn_config_default leaves it 0.
+   * pcdn_create refuses (PCDN_EINVAL) a non-zero value together with PCDN_FLAG_SHARED_PAYLOAD, a value
+   * above 0x1FFFFFFF, and a value whose largest copied record, round_up(4 + ref_min_bytes - 1, 32) bytes,
+   * does not fit an empty ring (ring_bytes_per_conn; with PCDN_FLAG_OUTPUT_POOL: the pool).  So with the
+   * threshold set, no message overflows a connection by its size alone: only a connection that does not
+   * drain its ring can overflow.                                                                   */
+  uint32_t ref_min_bytes;
 } pcdn_config;
 
 /* pcdn_config.ingest — sharded engines: how the staged batch gets from the host into every GPU */
@@ -448,10 +463,11 @@ int pcdn_receive_frames(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, in
 int pcdn_flush(pcdn_engine* e, uint64_t* batch_id);
 /* Submit an explicit ordered batch (R9: batch order = per-connection delivery order). */
 int pcdn_submit(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n, uint64_t* batch_id);
-/* Same, inputs already resident in HBM (no host copy, no host parse).  PCDN_FLAG_SHARED_PAYLOAD: the
- * frame arena is copied once into the slot's pinned staging (pcdn_batch_payload) before the batch
- * runs, and polling the batch waits for that copy; an arena larger than that staging
- * (max_batch_bytes) is PCDN_ENOSPC. */
+/* Same, inputs already resident in HBM (no host copy, no host parse).  PCDN_FLAG_SHARED_PAYLOAD or a
+ * non-zero ref_min_bytes: the frame arena is copied once into the slot's pinned staging
+ * (pcdn_batch_payload) before the batch runs, on the batch's stream (the main stream of the first local
+ * shard), and polling the batch waits for that copy; an arena larger than that staging (max_batch_bytes)
+ * is PCDN_ENOSPC. */
 int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* batch, uint64_t* batch_id);
 
 /* ---- data out: replaces Connection::send_message_raw + the per-connection writer task
@@ -462,13 +478,13 @@ int pcdn_next_batch(pcdn_engine* e, uint64_t* batch_id);
 /* Wait for (block != 0) or test a batch; fills *out (span table is in pinned host memory). */
 int pcdn_poll(pcdn_engine* e, uint64_t batch_id, pcdn_batch_result* out, int block);
 /* Copy `len` ring bytes of a connection to host memory: its records, as a socket writer walks them
- * (PCDN_FLAG_SHARED_PAYLOAD: reference records, resolved through pcdn_batch_payload).
+ * (PCDN_FLAG_SHARED_PAYLOAD or ref_min_bytes: reference records, resolved through pcdn_batch_payload).
  * With PCDN_FLAG_HOST_RINGS this is a plain memcpy; prefer pcdn_host_rings() and read in place.  */
 int pcdn_read(pcdn_engine* e, pcdn_conn conn, uint32_t ring_off, uint32_t len, void* dst);
 /* Pinned host memory holding the frames of a batch: a reference record's raw bytes are at
  * *host_base + its offset.  Valid until pcdn_release_batch of that batch; PCDN_ENOENT for an unknown or
  * released batch, and for a device-resident batch (pcdn_submit_device) of an engine without
- * PCDN_FLAG_SHARED_PAYLOAD, whose frames never reach the host.  Sharded engines and multi-process
+ * PCDN_FLAG_SHARED_PAYLOAD or ref_min_bytes, whose frames never reach the host.  Sharded engines and multi-process
  * groups return this process's own staged copy (identical everywhere by the SPMD contract).       */
 int pcdn_batch_payload(pcdn_engine* e, uint64_t batch_id, const uint8_t** host_base);
 /* PCDN_FLAG_OUTPUT_POOL: run a refused batch (status PCDN_EAGAIN) again after older batches have been
@@ -518,7 +534,7 @@ int pcdn_poll_shard(pcdn_engine* e, uint64_t batch_id, uint32_t local_shard, pcd
  * skipped, per-connection order kept — on a small thread pool; a failed write detaches the
  * connection and reports it (pcdn_egress_failed), the analogue of the reference removing a peer
  * whose send failed (cdn-broker/src/tasks/user/sender.rs:24-30).
- * PCDN_FLAG_SHARED_PAYLOAD: the chunks carry the reference records as stored; the fd sink sends each
+ * PCDN_FLAG_SHARED_PAYLOAD or ref_min_bytes: the chunks carry the reference records as stored; the fd sink sends each
  * as two iovecs (the 4 length bytes of the record, the L payload bytes from pcdn_batch_payload), and a
  * callback sink resolves them the same way through pcdn_batch_payload of the batch it drains.
  * Backlogs (backlog_bytes_per_conn / backlog_bytes_total, opt-in): without them a socket that cannot
@@ -596,7 +612,7 @@ int pcdn_set_timing(pcdn_engine* e, int on);
 int pcdn_ring_info(pcdn_engine* e, void** dev_base, uint64_t* ring_bytes, uint32_t* max_conns);
 /* PCDN_FLAG_HOST_RINGS: host address of the rings (valid for the life of the engine); NULL and
  * PCDN_ENOENT when the rings live in device memory.  The rings hold records (with
- * PCDN_FLAG_SHARED_PAYLOAD: reference records, see above). */
+ * PCDN_FLAG_SHARED_PAYLOAD or ref_min_bytes: reference records, see above). */
 int pcdn_host_rings(pcdn_engine* e, const void** host_base);
 /* number of connected users (Connections::num_users mod.rs:127) and brokers */
 int pcdn_num_users(pcdn_engine* e, uint32_t* users, uint32_t* brokers);

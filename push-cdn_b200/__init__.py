@@ -92,7 +92,7 @@ class Config(C.Structure):
         ("flags", C.c_uint32),
         ("n_devices", C.c_uint32), ("ingest", C.c_uint32), ("devices", C.POINTER(C.c_int32)),
         ("world_shards", C.c_uint32), ("first_shard", C.c_uint32), ("nccl_unique_id", C.c_void_p),
-        ("pool_bytes", C.c_uint64), ("global_memory_pool_size", C.c_uint64),
+        ("pool_bytes", C.c_uint64), ("global_memory_pool_size", C.c_uint64), ("ref_min_bytes", C.c_uint32),
     ]
 
 
@@ -310,7 +310,9 @@ class Engine:
     def __init__(self, device: int = 0, stream: Optional[int] = None, identity: str = "/",
                  devices: Optional[Sequence[int]] = None, nccl_unique_id: Optional[bytes] = None, **kw):
         """devices=[0, 1, ...]: one connection shard per listed GPU (the engine stays one logical
-        broker); world_shards / first_shard / nccl_unique_id: multi-process groups (see the header)."""
+        broker); world_shards / first_shard / nccl_unique_id: multi-process groups (see the header).
+        Any other keyword sets the pcdn_config field of that name, e.g. ref_min_bytes=16384: messages of
+        at least that many raw bytes are delivered by reference, shorter ones as framed copies."""
         self.L = lib()
         cfg = Config()
         self.L.pcdn_config_default(C.byref(cfg))
@@ -556,6 +558,10 @@ class Engine:
         self._chk(self.L.pcdn_read(self.h, conn, ring_off, length, C.cast(buf, C.c_void_p)))
         return buf.raw[:length]
 
+    def delivers_by_ref(self) -> bool:
+        """some deliveries are reference records (FLAG_SHARED_PAYLOAD, or a ref_min_bytes threshold)"""
+        return bool(self.cfg.flags & FLAG_SHARED_PAYLOAD) or self.cfg.ref_min_bytes > 0
+
     def batch_payload(self, batch_id: int) -> int:
         """host address of the batch's frames (pinned, valid until release): a reference record's raw
         bytes are at this address + the record's offset"""
@@ -585,7 +591,7 @@ class Engine:
     def collect_frames(self, res: BatchResult) -> Dict[int, List[bytes]]:
         """What the per-connection writer tasks would put on the wire for this batch: walk every
         span record by record (BE length prefix, 32-byte record stride; a reference record of a
-        FLAG_SHARED_PAYLOAD engine is resolved through batch_payload) and return the raw frames
+        FLAG_SHARED_PAYLOAD or ref_min_bytes engine is resolved through batch_payload) and return the raw frames
         per connection in ring order.  A wrapped connection has two spans: the one that does not
         start at offset 0 comes first."""
         per: Dict[int, List[Tuple[int, int, int]]] = {}
@@ -593,8 +599,8 @@ class Engine:
         stride, rbytes = sh[0].shard_stride, sh[0].ring_bytes
         hosts = {d.global_index: d.rings_host for d in sh if d.rings_host}
         pool = bool(self.cfg.flags & FLAG_OUTPUT_POOL)   # offsets: 32-byte units relative to res.pool_base
-        # shared-payload engines: reference records point into the batch's payload
-        payload = self.batch_payload(res.batch_id) if self.cfg.flags & FLAG_SHARED_PAYLOAD else 0
+        # engines that deliver by reference: reference records point into the batch's payload
+        payload = self.batch_payload(res.batch_id) if self.delivers_by_ref() else 0
         for conn, off, ln, nrec in self.spans(res):
             per.setdefault(conn, []).append((off, ln, nrec))
         out: Dict[int, List[bytes]] = {}

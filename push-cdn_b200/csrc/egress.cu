@@ -11,8 +11,9 @@
 // c-1), and the sink gets {host bytes, spans, offset of every span}.  Engines with PCDN_FLAG_HOST_RINGS
 // skip all of that: the sink sees the rings in place.  The built-in sink writes every span to the
 // file descriptor attached to its connection with writev (length prefix + raw bytes per record, the
-// padding between records skipped), on a small thread pool, keeping per-connection order.  On a
-// PCDN_FLAG_SHARED_PAYLOAD engine a reference record becomes two iovecs: its 4 length bytes and the L
+// padding between records skipped), on a small thread pool, keeping per-connection order.  On an engine
+// that delivers by reference (PCDN_FLAG_SHARED_PAYLOAD, or messages of at least ref_min_bytes) a reference
+// record becomes two iovecs: its 4 length bytes and the L
 // bytes of the batch's payload (pcdn_batch_payload) it points to.
 //
 // With backlogs configured (pcdn_egress_config.backlog_bytes_*) the built-in sink never waits for a
@@ -167,7 +168,7 @@ struct pcdn_egress {
   std::vector<pcdn_conn> failed, failed_out;
   pcdn_egress_stats last{};
   std::atomic<uint64_t> fd_bytes{0}, fd_writes{0}, unattached{0}, records{0};
-  // PCDN_FLAG_SHARED_PAYLOAD: the batch being drained and its payload base (reference records point into it)
+  // engines that deliver by reference: the batch being drained and its payload base (reference records point into it)
   const uint8_t* payload = nullptr;
   uint64_t batch_id = 0;
   std::atomic<bool> bad_ref{false};
@@ -547,7 +548,7 @@ int drain_locked(pcdn_egress* g, uint64_t batch_id, pcdn_egress_sink sink, void*
   const uint32_t nl = (uint32_t)e->shards.size();
   int rc = 0;
   g->payload = nullptr; g->batch_id = batch_id; g->bad_ref = false;
-  if ((e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) && (rc = pcdn_batch_payload(e, batch_id, &g->payload))) return rc;
+  if (e->delivers_by_ref() && (rc = pcdn_batch_payload(e, batch_id, &g->payload))) return rc;
   if (nl == 1) {
     rc = drain_shard(g, batch_id, 0, sink, user, &st);
   } else {

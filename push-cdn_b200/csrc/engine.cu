@@ -106,7 +106,7 @@ int flush_journal(pcdn_engine* e) {
 }
 
 void slot_reset_open(Slot& s) {
-  s.arena_used = 0; s.n_direct = 0; s.devparse = false; s.ingress_bytes = 0; s.n_msgs = 0;
+  s.arena_used = 0; s.n_direct = 0; s.devparse = false; s.ingress_bytes = 0; s.n_msgs = 0; s.max_raw_len = 0;
   s.kind.clear(); s.flags.clear(); s.slot_off16.clear(); s.raw_len.clear(); s.aux_off.clear(); s.aux_len.clear();
   s.bcast_index.clear(); s.topics.clear(); s.events.clear(); s.ev_topics.clear();
   s.device_input = false; s.counted = false;
@@ -191,7 +191,8 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
       const ShardSlot& o = sh.slots[pv];
       if (cudaEventQuery(o.ev_done) != cudaSuccess) { cudaGetLastError(); continue; }
       const BatchStats& ps_ = *o.h_stats;
-      sh.fat_only = ps_.status == 0 && ps_.n_cm == 0 && ps_.n_fat_tiles > 0 && ps_.bytes_out <= kOverlapMaxBytes;
+      // (message-major entries, not tiles: a message delivered by reference has its entries but no tile)
+      sh.fat_only = ps_.status == 0 && ps_.n_cm == 0 && ps_.n_fat_entries > 0 && ps_.bytes_out <= kOverlapMaxBytes;
       break;
     }
   }
@@ -269,7 +270,11 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   if (!((pack_variant >> 8) & 15u)) pack_variant |= (fat_overlap ? 3u : 4u) << 8;
   // the final counters reach h_stats from the last pack kernel (mapped memory, covered by ev_done); only a
   // batch without a pack launch copies them
-  const bool published = launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, fused ? nullptr : s.d_stats_pub, ps);
+  // engines with ref_min_bytes: a host-staged batch runs k_pack_ref only when a message reaches the threshold; the
+  // lengths of a device-resident batch are on the device, so it always does
+  const Slot& hs = e->slots[si];
+  const bool has_ref = e->cfg.ref_min_bytes && (hs.device_input || hs.max_raw_len >= e->cfg.ref_min_bytes);
+  const bool published = launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, has_ref, fused ? nullptr : s.d_stats_pub, ps);
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[5], ps));
   CUDA_TRY(cudaGetLastError());
   if (!fused && !published) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));
@@ -454,13 +459,16 @@ struct BatchFill {
   uint32_t msgs = 0, bcast = 0;
   uint64_t bytes = 0, topics = 0, ingress = 0;
   uint64_t ev_topics = 0;   // topic entries of the batch's subscription events (they share the topic capacity)
+  uint32_t max_raw_len = 0;
   void add(const MsgShape& m) {
     msgs++; bcast += m.kind == PCDN_KIND_BROADCAST ? 1 : 0;
     bytes += m.bytes(); topics += m.n_topics; ingress += m.raw_len;
+    max_raw_len = std::max(max_raw_len, m.raw_len);
   }
 };
 BatchFill fill_of(const Slot& s) {
-  return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0, s.ev_topics.size()};
+  return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0, s.ev_topics.size(),
+                   s.max_raw_len};
 }
 
 // The per-batch limits: nullptr when `m` still fits a batch that holds `f`, else the limit it would
@@ -584,7 +592,7 @@ void write_msg(Slot& s, uint32_t mi, size_t off, uint32_t aux_off, uint32_t bcas
 
 // the open slot `s` now holds `f`: messages up to f.msgs are written
 void slot_commit(pcdn_engine* e, Slot& s, const BatchFill& f, bool devparse) {
-  s.arena_used = f.bytes; s.n_direct = f.msgs - f.bcast; s.devparse |= devparse;
+  s.arena_used = f.bytes; s.n_direct = f.msgs - f.bcast; s.devparse |= devparse; s.max_raw_len = f.max_raw_len;
   s.ingress_bytes += f.ingress; e->inflight_bytes += f.ingress; e->stats.bytes_in += f.ingress;
 }
 
@@ -721,7 +729,7 @@ int init_shard(pcdn_engine* e, Shard& sh, int ndev, void* user_stream) {
   d.N = Ns; d.W = Ws; d.T = g.T; d.nblk = Ws / kBlockWords;
   d.bucket_mask = g.bucket_mask; d.key_stride = g.key_stride; d.seed = g.seed;
   d.ring_bytes = c.ring_bytes_per_conn; d.ring_units = (uint32_t)(c.ring_bytes_per_conn / kUnit);
-  d.shared_payload = (c.flags & PCDN_FLAG_SHARED_PAYLOAD) ? 1u : 0u;
+  d.ref_min = (c.flags & PCDN_FLAG_SHARED_PAYLOAD) ? 0u : c.ref_min_bytes ? c.ref_min_bytes : 0xFFFFFFFFu;
   d.n_valid_topics = c.n_valid_topics;
   d.max_key_len = c.max_key_len;
   d.conn_base = sh.gindex * Ns;
@@ -927,7 +935,16 @@ void pcdn_config_default(pcdn_config* c) {
 int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
   GUARD_BEGIN
   if (!cfg || !out) return fail(PCDN_EINVAL, "null argument");
-  if (cfg->struct_size != sizeof(pcdn_config)) return fail(PCDN_EINVAL, "pcdn_config.struct_size mismatch (ABI)");
+  // a config of the size before ref_min_bytes existed: the field is 0 (every delivery a framed copy)
+  constexpr uint32_t kNoRefMinSize = offsetof(pcdn_config, ref_min_bytes);
+  if (cfg->struct_size != sizeof(pcdn_config) && cfg->struct_size != kNoRefMinSize)
+    return fail(PCDN_EINVAL, "pcdn_config.struct_size mismatch (ABI)");
+  if (cfg->struct_size == kNoRefMinSize) {
+    pcdn_config full{};
+    std::memcpy(&full, cfg, kNoRefMinSize);
+    full.struct_size = sizeof(pcdn_config);
+    return pcdn_create(&full, out);
+  }
   if (!cfg->max_conns || !cfg->max_topics || cfg->max_topics > 65536 || !cfg->max_keys || !cfg->max_key_len ||
       !cfg->max_batch_msgs || !cfg->batch_slots)
     return fail(PCDN_EINVAL, "zero or out-of-range capacity in pcdn_config");
@@ -937,6 +954,9 @@ int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
   if (cfg->max_key_len > 4096) return fail(PCDN_EINVAL, "max_key_len > 4096");
   if (cfg->pack_variant & ~0xFF00u)
     return fail(PCDN_EINVAL, "pack_variant: only the CTA-count fields remain (bits 8-11: k_pack, bits 12-15: k_pack_direct CTAs per SM)");
+  if (cfg->ref_min_bytes && (cfg->flags & PCDN_FLAG_SHARED_PAYLOAD))
+    return fail(PCDN_EINVAL, "ref_min_bytes and PCDN_FLAG_SHARED_PAYLOAD exclude each other (the flag delivers every message by reference)");
+  if (cfg->ref_min_bytes > 0x1FFFFFFFu) return fail(PCDN_EINVAL, "ref_min_bytes above MAX_MESSAGE_SIZE (0x1FFFFFFF)");
   // ---- connection shards
   const uint32_t n_local = cfg->n_devices ? cfg->n_devices : 1;
   const uint32_t world = cfg->world_shards ? cfg->world_shards : n_local;
@@ -989,6 +1009,16 @@ int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
     if (e->pool_bytes < 4096 || e->pool_bytes / PCDN_RECORD_ALIGN >= 0xFFFFFFFFull) {
       delete e;
       return fail(PCDN_EINVAL, "pool_bytes must be between 4 KiB and 128 GiB");
+    }
+  }
+  if (cfg->ref_min_bytes) {
+    // the largest record still copied must fit an empty ring (the pool): then no message overflows by its size alone
+    const uint64_t largest_copy = align_up(4 + (uint64_t)cfg->ref_min_bytes - 1, PCDN_RECORD_ALIGN);
+    const bool pool = (cfg->flags & PCDN_FLAG_OUTPUT_POOL) != 0;
+    if (largest_copy > (pool ? e->pool_bytes : cfg->ring_bytes_per_conn)) {
+      delete e;
+      return fail(PCDN_EINVAL, pool ? "ref_min_bytes: the largest copied record (4 + ref_min_bytes - 1, 32-byte aligned) exceeds pool_bytes"
+                                    : "ref_min_bytes: the largest copied record (4 + ref_min_bytes - 1, 32-byte aligned) exceeds ring_bytes_per_conn");
     }
   }
   e->tables.reset(new HostTables(g));
@@ -1510,7 +1540,7 @@ int pcdn_submit_device(pcdn_engine* e, const pcdn_device_batch* b, uint64_t* bat
       b->n_bcast > b->n_msgs)
     return fail(PCDN_EINVAL, "device batch exceeds configured capacities");
   const uint32_t n = b->n_msgs, nb = b->n_bcast;
-  const bool shared = (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) != 0;
+  const bool shared = e->delivers_by_ref();   // the frames are staged on the host as the payload of reference records
   if (shared && b->arena_bytes > e->frames_cap)
     return fail(PCDN_ENOSPC, "device batch frames exceed the pinned payload staging (max_batch_bytes)");
   // sharded engines: the frames at the start of a receiving shard's arena, the descriptor block behind them
@@ -1785,9 +1815,9 @@ int pcdn_batch_payload(pcdn_engine* e, uint64_t batch_id, const uint8_t** host_b
   if (si < 0) return fail(PCDN_ENOENT, "unknown or released batch id");
   const Slot& s = e->slots[si];
   // host-staged batches keep their frames in the slot's pinned staging until release; device-resident
-  // ones have them copied there only by shared-payload engines
-  if (s.device_input && !(e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD))
-    return fail(PCDN_ENOENT, "the frames of a device-resident batch are staged on the host only with PCDN_FLAG_SHARED_PAYLOAD");
+  // ones have them copied there only by engines that deliver by reference
+  if (s.device_input && !e->delivers_by_ref())
+    return fail(PCDN_ENOENT, "the frames of a device-resident batch are staged on the host only with PCDN_FLAG_SHARED_PAYLOAD or ref_min_bytes");
   if (host_base) *host_base = s.h_arena;
   return 0;
   GUARD_END
@@ -1835,7 +1865,7 @@ int pcdn_release_batch(pcdn_engine* e, uint64_t batch_id) {
     // its pinned staging buffers must not be refilled before that copy ran (device-input batches have
     // no host staging and stay fully asynchronous — the pipelined submit_device/release loop — unless
     // their frames are being copied into the staging as the shared payload: ev_done comes after that copy).
-    const bool payload_copy = s.device_input && (e->cfg.flags & PCDN_FLAG_SHARED_PAYLOAD);
+    const bool payload_copy = s.device_input && e->delivers_by_ref();
     if (!ss.polled && (!s.device_input || payload_copy))
       CUDA_TRY(cudaEventSynchronize((e->sharded && !payload_copy) ? ss.ev_ingest : ss.ev_done));
     // ring space may be reused only after the pack that filled it has finished

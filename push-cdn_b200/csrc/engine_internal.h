@@ -145,6 +145,7 @@ struct Slot {
   uint64_t ingress_bytes = 0;   // pool permits held by this batch
   std::chrono::steady_clock::time_point t_launch;
   bool devparse = false;        // some messages carry MSGF_DEVPARSE (k_parse runs first)
+  uint32_t max_raw_len = 0;     // host-staged: longest message (with ref_min_bytes: whether k_pack_ref runs)
   bool counted = false;         // counters of this batch have been added to the engine stats
   // merged view of a sharded batch for pcdn_poll (host copy of the shards' span tables)
   std::vector<pcdn_span> merged_spans;
@@ -200,6 +201,8 @@ struct pcdn_engine {
   std::vector<pcdn_topic_sync_entry> sync_topics_c;
 
   bool owns_root() const { return first_shard == 0; }   // this process holds global shard 0 (ingest root)
+  // some deliveries are reference records, resolved through the batch's host payload (pcdn_batch_payload)
+  bool delivers_by_ref() const { return (cfg.flags & PCDN_FLAG_SHARED_PAYLOAD) || cfg.ref_min_bytes; }
   uint32_t shard_N() const { return geo.shard_N; }
   uint32_t shard_W() const { return geo.shard_N / 32; }
 };

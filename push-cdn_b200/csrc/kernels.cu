@@ -539,10 +539,13 @@ void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats
 // =============================================================================== K1p plan
 __device__ __forceinline__ uint32_t frame_vec_bytes(uint32_t raw_len) { return (4u + raw_len + 15u) & ~15u; }
 __device__ __forceinline__ uint32_t frame_units(uint32_t raw_len) { return (4u + raw_len + kUnit - 1u) / kUnit; }
-// units one delivery takes in a ring / the output pool: the framed copy, or (PCDN_FLAG_SHARED_PAYLOAD)
-// one 32-byte reference record.  Every placement site (k_offsets, its direct path, k_ctrl_small) uses it.
+// The one delivery rule: a message is delivered by reference (one 32-byte record, k_pack_ref) when its raw
+// length reaches DevState::ref_min, else as a framed copy.  Shared payload: always; copy mode: never.
+__device__ __forceinline__ bool by_ref(const DevState& s, uint32_t raw_len) { return raw_len >= s.ref_min; }
+// units one delivery takes in a ring / the output pool: the framed copy, or one 32-byte reference record.
+// Every placement site (k_offsets, its direct path, k_ctrl_small) uses it.
 __device__ __forceinline__ uint32_t rec_units(const DevState& s, uint32_t raw_len) {
-  return s.shared_payload ? 1u : frame_units(raw_len);
+  return by_ref(s, raw_len) ? 1u : frame_units(raw_len);
 }
 // recipients per message-major tile: about kFatTileBytes of stores per tile whatever the frame size, so a
 // batch of large frames still splits into enough tiles to balance ~450 persistent CTAs
@@ -557,16 +560,17 @@ __device__ __forceinline__ void plan_classify(const DevState& s, const BatchIn& 
   uint32_t cls = CLS_THIN, tiles = 0;
   if (d >= kFatMin) {
     const uint32_t len = b.raw_len[m];
-    // (shared payload: every delivery is one 32-byte record with an explicit {conn, off} entry; the
-    //  connection-major class stages frame copies, so it is off)
-    const bool dense = !s.shared_payload && ((uint64_t)d << kCmDenseShift) >= s.N && b.kind[m] == 4;
+    // (by reference: every delivery is one 32-byte record with an explicit {conn, off} entry in efat, written by
+    //  k_pack_ref.  The connection-major class and the message-major tiles stage frame copies: neither applies.)
+    const bool ref = by_ref(s, len);
+    const bool dense = !ref && ((uint64_t)d << kCmDenseShift) >= s.N && b.kind[m] == 4;
     if (dense && frame_units(len) * kUnit <= kCmMaxBytes) {
       cls = CLS_CM;
     } else {
       cls = CLS_FAT;
       const uint32_t nch = (frame_vec_bytes(len) + kChunkBytes - 1) / kChunkBytes;
       const uint32_t tr = tile_recipients(frame_vec_bytes(len));
-      tiles = nch * ((d + tr - 1) / tr);
+      tiles = ref ? 0u : nch * ((d + tr - 1) / tr);
     }
   }
   *cls_out = cls; *tiles_out = tiles;
@@ -1366,7 +1370,8 @@ __device__ __forceinline__ void copy_record(const uint4* __restrict__ src, uint4
     if (p3) st_stream16(dst + v + 96, x3);
   }
 }
-// Warp per scatter-list entry (broadcasts with < kFatMin recipients).
+// Warp per scatter-list entry (broadcasts with < kFatMin recipients); k_pack_ref writes the entries of
+// messages delivered by reference.
 __device__ __forceinline__ void pack_thin_phase(const DevState& s, const BatchIn& b, const Work& w) {
   const uint32_t n = w.stats->n_thin_entries;
   const uint32_t pool_base = w.stats->pool_base;
@@ -1374,7 +1379,7 @@ __device__ __forceinline__ void pack_thin_phase(const DevState& s, const BatchIn
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t e = gw; e < n; e += nw) {
     const uint4 ent = w.ethin[e];
-    if (ent.y == kOffInvalid) continue;
+    if (ent.y == kOffInvalid || by_ref(s, ent.w)) continue;
     copy_record(reinterpret_cast<const uint4*>(b.arena + (size_t)ent.z * 16),
                 reinterpret_cast<uint4*>(conn_out(s, w, ent.x, pool_base) + (size_t)ent.y * kUnit), ent.w, lane);
   }
@@ -1399,7 +1404,7 @@ __device__ __forceinline__ void pack_direct_phase(const DevState& s, const Batch
     const uint32_t cso = so, clen = len;
     const uint32_t nx = m + nw;
     if (nx < n) { ent = w.edir[nx]; so = b.slot_off16[nx]; len = b.raw_len[nx]; }
-    if (cur.y == kOffInvalid) continue;
+    if (cur.y == kOffInvalid || by_ref(s, clen)) continue;   // (by reference: k_pack_ref)
     copy_record(reinterpret_cast<const uint4*>(b.arena + (size_t)cso * 16),
                 reinterpret_cast<uint4*>(conn_out(s, w, cur.x, pool_base) + (size_t)cur.y * kUnit), clen, lane);
   }
@@ -1455,8 +1460,9 @@ __global__ void __launch_bounds__(256, 8) k_pack_direct(DevState s, BatchIn b, W
 }
 
 // =============================================================================== K2r pack (reference records)
-// PCDN_FLAG_SHARED_PAYLOAD: every delivery is ONE 32-byte reference record (pcdn_fanout.h) instead of a
-// framed copy: marker, BE length, offset of the raw bytes in the batch's frame arena, batch id, zero.
+// A message delivered by reference (by_ref: every message of a PCDN_FLAG_SHARED_PAYLOAD engine, those of at
+// least ref_min_bytes on an engine with that threshold) gets ONE 32-byte reference record (pcdn_fanout.h) per
+// delivery instead of a framed copy: marker, BE length, offset of the raw bytes in the batch's frame arena, batch id, zero.
 // One sector, two 16-byte streaming stores, no partial-sector write.  The record depends on the message
 // and the batch only, so a retried batch writes identical records wherever the pool places them.
 __device__ __forceinline__ void st_ref_record(uint8_t* dst, uint32_t raw_len, uint32_t slot_off16, unsigned long long batch_id) {
@@ -1467,7 +1473,8 @@ __device__ __forceinline__ void st_ref_record(uint8_t* dst, uint32_t raw_len, ui
 // Thread per delivery over the three scatter lists back to back: message-major (efat: the owning message
 // is found by a binary search of eb_fat), thin (ethin carries everything) and direct (edir, entry m =
 // message m).  Entries of one message are in connection order, so a warp's 32 stores go to 32
-// consecutive connections; a connection's records of successive messages are adjacent in its ring.
+// consecutive connections; a connection's records of successive messages are adjacent in its ring.  Entries of
+// messages delivered as copies are k_pack's: skipped here (never on a shared-payload engine).
 __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w, int do_direct, BatchStats* publish) {
   if (w.stats->status) { publish_if_last(w, publish); return; }
   const uint32_t nfat = w.stats->n_fat_entries, nthin = w.stats->n_thin_entries;
@@ -1494,6 +1501,9 @@ __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w,
     }
     if (off == kOffInvalid) continue;   // ring overflow, or a direct message this shard does not deliver
     if (!thin) { slot = b.slot_off16[m]; len = b.raw_len[m]; }
+    // (a copied message's entries are k_pack's; those of a connection-major one are not even in efat, whose
+    //  slots in its range hold nothing meaningful: this test comes before conn / off are used)
+    if (!by_ref(s, len)) continue;
     st_ref_record(conn_out(s, w, conn, pool_base) + (size_t)off * kUnit, len, slot, bid);
   }
   publish_if_last(w, publish);
@@ -1504,21 +1514,28 @@ __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w,
 // direct pack (default 8 = full occupancy).  Neither changes what is written, only how the persistent
 // CTAs share the work.
 bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
-                 BatchStats* publish, cudaStream_t st) {
-  if (s.shared_payload) {   // (the CTA counts of pack_variant describe k_pack and k_pack_direct: they do not apply here)
+                 bool has_ref, BatchStats* publish, cudaStream_t st) {
+  // (the CTA counts of pack_variant describe k_pack and k_pack_direct: they do not apply to k_pack_ref)
+  const uint32_t ref_ctas = (uint32_t)n_sms * 8;
+  if (s.ref_min == 0) {   // shared payload: k_pack_ref is the whole pack
     if (!b.n_bcast && !n_direct) return false;
-    PCDN_COUNT_LAUNCH, k_pack_ref<<<(uint32_t)n_sms * 8, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
+    PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_ctas, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
     return true;
   }
+  // copies; with a message delivered by reference in the batch, k_pack_ref follows on the same stream and is the
+  // kernel that publishes the counters
+  BatchStats* copy_publish = has_ref ? nullptr : publish;
   const bool direct_separate = n_direct >= kThinSeparateMin;
   const uint32_t ctas_per_sm = ((pack_variant >> 8) & 15u) ? ((pack_variant >> 8) & 15u) : 3;
   const uint32_t grid = (uint32_t)n_sms * ctas_per_sm;
   const int do_direct = (n_direct && !direct_separate) ? 1 : 0;
   if (b.n_bcast || do_direct)  // (a batch of nothing but many direct messages has no work for this kernel)
-    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct, direct_separate ? nullptr : publish);
+    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct, direct_separate ? nullptr : copy_publish);
   const uint32_t dctas = ((pack_variant >> 12) & 15u) ? ((pack_variant >> 12) & 15u) : 8u;
-  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w, publish);
-  return direct_separate || b.n_bcast || do_direct;
+  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w, copy_publish);
+  const bool launched = direct_separate || b.n_bcast || do_direct;
+  if (has_ref && launched) PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_ctas, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
+  return launched;
 }
 
 // =============================================================================== release

@@ -19,8 +19,9 @@
 //                       ~128 KB worth of recipients per tile), thin (warp per delivery), direct (warp
 //                       per message; its own full-occupancy launch k_pack_direct for batches of >= 2048
 //                       direct messages)
-//   K2r k_pack_ref      (PCDN_FLAG_SHARED_PAYLOAD) replaces K2: thread per delivery over the three scatter
-//                       lists, one 32-byte reference record each (the payload stays once per batch)
+//   K2r k_pack_ref      thread per delivery over the three scatter lists, one 32-byte reference record for each
+//                       delivery of a by-reference message (the payload stays once per batch).  Replaces K2 on
+//                       PCDN_FLAG_SHARED_PAYLOAD engines; follows K2 on engines with a ref_min_bytes threshold
 //   K1s k_ctrl_small    latency path (N <= 65536 connection slots, <= 256 messages): K3 + sort + K1a +
 //                       K1p + K1b in ONE cluster launch, counters/spans published to mapped host memory
 //   K4  k_apply_*       scatter of changed table words/slots (subscribe, add/remove, direct map)
@@ -99,7 +100,10 @@ struct DevState {
   uint32_t conn_base;
   uint32_t span_runs;    // PCDN_FLAG_SPAN_RUNS: the span table is run-length encoded (SpanRun entries)
   uint32_t count_drops;  // 1 on exactly one shard of the broker (global shard 0): it counts the unroutable directs
-  uint32_t shared_payload;  // PCDN_FLAG_SHARED_PAYLOAD: one 32-byte reference record per delivery (k_pack_ref), no cm class
+  // a message of raw_len >= ref_min is delivered as one 32-byte reference record (k_pack_ref), a shorter one as a
+  // framed copy (kernels.cu: by_ref): 0 = every message (PCDN_FLAG_SHARED_PAYLOAD), 0xFFFFFFFF = none (copy mode),
+  // else pcdn_config.ref_min_bytes
+  uint32_t ref_min;
   uint64_t ring_bytes;
 };
 
@@ -248,9 +252,10 @@ void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool 
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);
 // publish (mapped host memory): the last pack kernel copies the batch's final counters there; returns false when
-// the batch launches no pack kernel, so nothing was published
+// the batch launches no pack kernel, so nothing was published.  has_ref: the batch may hold a message delivered by
+// reference (engines with a threshold launch k_pack_ref after the copy packs; shared-payload engines ignore it)
 bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
-                 BatchStats* publish, cudaStream_t st);
+                 bool has_ref, BatchStats* publish, cudaStream_t st);
 void launch_release(const DevState& s, const uint32_t* batch_units, const BatchStats* stats, cudaStream_t st);
 void launch_pool_init(const DevState& s, cudaStream_t st);
 unsigned long long kernel_launches();   // launches issued by this library in this process so far
