@@ -126,8 +126,9 @@ typedef struct pcdn_config {
   uint64_t global_memory_pool_size; /* Limiter analogue (cdn-proto/src/connection/limiter/mod.rs:56-68,
                                  * cdn-broker/src/binaries/broker.rs:71-72 default 1 GiB): bytes of inbound frames
                                  * that may be in flight (accepted, their batch not yet released); 0 = unlimited.
-                                 * The reference awaits the semaphore; here a frame that does not fit is refused
-                                 * with PCDN_EAGAIN and the caller retries after releasing a batch. */
+                                 * The reference awaits the semaphore; here a frame that does not fit launches the
+                                 * open batch and is refused with PCDN_EAGAIN: the caller retries after releasing a
+                                 * batch (the launched one holds the permits it would wait for). */
   /* Delivery by reference above a size threshold: a routed message (broadcast or direct) whose raw length is
    * >= ref_min_bytes is delivered as ONE reference record per recipient (the layout of
    * PCDN_FLAG_SHARED_PAYLOAD below, its payload resolved through pcdn_batch_payload); every shorter message
@@ -423,8 +424,11 @@ int pcdn_broker_receive(pcdn_engine* e, const char* identifier, const uint8_t* r
  * The callback runs on the thread that calls pcdn_user_receive / pcdn_broker_receive /
  * pcdn_receive_frames, with the engine lock held: it must not call back into the same engine.
  * A hooked origin is always parsed on the host: PCDN_FLAG_DEVICE_PARSE is bypassed for its frames
- * (the device parser never shows a message to the host) and pcdn_receive_frames takes its
- * sequential path.  pcdn_handle_*_message / pcdn_submit are below the hook, as in the reference.   */
+ * (the device parser never shows a message to the host).  While a hook is set, pcdn_receive_frames
+ * parses each frame on the calling thread when it comes to it, so the hook sees the frames in order:
+ * those the call consumes and the one it stops at, if it stops early (that frame is shown again when
+ * the caller retries it).  pcdn_handle_*_message / pcdn_submit are below the hook, as in the
+ * reference.                                                                                        */
 enum { PCDN_HOOK_PROCESS = 0, PCDN_HOOK_SKIP = 1 };  /* HookResult; any negative return = Err */
 typedef struct pcdn_hook_message {
   uint8_t kind;             /* PCDN_KIND_*                                                          */
@@ -445,7 +449,8 @@ int pcdn_set_message_hook(pcdn_engine* e, int origin, pcdn_message_hook cb, void
 
 /* Many inbound frames in one call (one lock, no per-call FFI cost): frame i enters
  * user_receive_loop (origin 0, `sender` = that user's key) or broker_receive_loop (origin 1).
- * rc_out[i] (optional) gets what pcdn_user_receive / pcdn_broker_receive would have returned.
+ * rc_out[i] (optional) gets what pcdn_user_receive / pcdn_broker_receive would have returned for
+ * frame i, and pcdn_last_error is left as those calls, one per frame, would have left it.
  * Returns the number of frames consumed (== n unless a capacity condition — no free batch slot,
  * global memory pool exhausted — stopped it: drain a batch and call again with the rest) or a
  * negative code when not even the first frame could be taken.  Large calls are parsed and copied

@@ -434,26 +434,6 @@ int before_state_change(pcdn_engine* e) {
   return rc;
 }
 
-// One message on its way into a batch (an aggregate: InMsg{} is the empty message).
-struct InMsg {
-  uint8_t kind, flags;
-  bool prune;                        // broadcast: apply Topic::prune to the wire topic list
-  uint32_t raw_len, key_len;         // key_len: direct message's recipient length (routed_key_len)
-  uint32_t n_listed, n_topics;       // broadcast: entries of the topic list below, entries it adds to the batch
-  const uint8_t* raw;
-  const uint8_t* key;                // direct: the recipient
-  const uint16_t* topic_ids;         // broadcast: the topic ids (API calls), or null and
-  const uint8_t* wire_topics;        // a frame's wire topic list, pruned or verbatim
-};
-
-// What one message adds to a batch: a 16-byte frame slot (4-byte length hole, raw bytes, zero pad),
-// `key_bytes` of recipient key staged beside it (0 when the key is read in place) and topic entries.
-struct MsgShape {
-  uint8_t kind;
-  uint32_t raw_len, key_bytes, n_topics;
-  size_t bytes() const { return align_up(4 + (size_t)raw_len, 16) + key_bytes; }
-};
-
 // What a batch holds.  `ingress`: bytes admitted to it that e->inflight_bytes does not count yet.
 struct BatchFill {
   uint32_t msgs = 0, bcast = 0;
@@ -496,20 +476,17 @@ int apply_sub(pcdn_engine* e, SubOp op, const std::string& who, const uint16_t* 
   }
 }
 
-// PCDN_FLAG_INBATCH_SUBSCRIBE: the open batch (opened here when there is none), holding `f`, takes one
-// more event of n topics
-bool event_fits(pcdn_engine* e, const BatchFill& f, uint32_t n) {
-  if (!(e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) || e->open_slot < 0) return false;
-  const Slot& s = e->slots[e->open_slot];
-  return s.events.size() < e->cfg.max_batch_msgs && f.topics + f.ev_topics + n <= e->topics_cap;
-}
-
-// `op` as an event of the open batch at position `pos`: the mirror changes now, the device bitmap keeps
-// the words' values before the batch's events until its control kernels have run (HostTables::hold), and
-// the batch's match replays the event on the messages at or after `pos` (kernels.cu: apply_events)
-int record_event(pcdn_engine* e, uint32_t pos, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n) {
+// PCDN_FLAG_INBATCH_SUBSCRIBE: `op` as an event of the open batch, which holds `f`, at position f.msgs —
+// or 1 when the batch cannot take one more event of n topics.  The mirror changes now, the device bitmap
+// keeps the words' values before the batch's events until its control kernels have run (HostTables::hold),
+// and the batch's match replays the event on the messages at or after f.msgs (kernels.cu: apply_events)
+int record_event(pcdn_engine* e, const BatchFill& f, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n) {
   HostTables& t = *e->tables;
   Slot& s = e->slots[e->open_slot];
+  if (!(e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) || s.events.size() >= e->cfg.max_batch_msgs ||
+      f.topics + f.ev_topics + n > e->topics_cap)
+    return 1;
+  const uint32_t pos = f.msgs;
   uint32_t conn;
   t.hold = true;
   const int rc = apply_sub(e, op, who, topics, n, &conn);
@@ -525,11 +502,10 @@ int record_event(pcdn_engine* e, uint32_t pos, SubOp op, const std::string& who,
 // A subscription change from the C ABI or a user's Subscribe / Unsubscribe frame: an event of the open
 // batch when the flag is set and it fits there, else (R12) the open batch is launched first
 int sub_change(pcdn_engine* e, SubOp op, const std::string& who, const uint16_t* topics, uint32_t n) {
-  int rc;
-  if ((e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) && (e->open_slot >= 0 || acquire_open_slot(e) == 0) &&
-      event_fits(e, fill_of(e->slots[e->open_slot]), n)) {
-    rc = record_event(e, (uint32_t)e->slots[e->open_slot].kind.size(), op, who, topics, n);
-  } else {
+  int rc = 1;
+  if ((e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) && (e->open_slot >= 0 || acquire_open_slot(e) == 0))
+    rc = record_event(e, fill_of(e->slots[e->open_slot]), op, who, topics, n);
+  if (rc == 1) {
     if ((rc = before_state_change(e))) return rc;
     uint32_t conn;
     rc = apply_sub(e, op, who, topics, n, &conn);
@@ -555,14 +531,106 @@ bool pool_admits(const pcdn_engine* e, uint64_t bytes) {
 // would not do: that is the key of a user whose key is empty.)
 uint32_t routed_key_len(const pcdn_engine* e, uint32_t len) { return len > e->cfg.max_key_len ? e->cfg.max_key_len + 1 : len; }
 
-// a message of the C ABI's handle / submit calls
-InMsg api_msg(const pcdn_engine* e, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
-              const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw, uint32_t raw_len) {
-  InMsg m{};
+// Entry `p` as the `batch` entry of message `m`.  A direct message's recipient is read in place when it lies
+// inside the frame at a 4-byte aligned offset (the frame starts 4 bytes into a 16-byte slot), else (and
+// whenever the caller set m.stage_key) it is staged beside the frame.
+void as_batch(Entry& p, InMsg& m) {
+  if (m.kind == PCDN_KIND_DIRECT)
+    m.stage_key |= !(m.key && m.key >= m.raw && m.key + m.key_len <= m.raw + m.raw_len && ((m.key - m.raw) & 3) == 0);
+  p.route = ROUTE_BATCH; p.devparse = (m.flags & MSGF_DEVPARSE) != 0; p.rc = 0; p.why = nullptr;
+  p.shape = MsgShape{m.kind, m.raw_len, m.stage_key ? (uint32_t)align_up(m.key_len, 16) : 0u, m.n_topics};
+}
+
+// Scratch entry i as a message of the C ABI's handle / submit calls.  A multi-process group stages every
+// recipient of these calls: the layout must not depend on how a process happens to hold the bytes (a
+// parsed frame's recipient lies at the same offset in every process).
+void api_entry(pcdn_engine* e, uint32_t i, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
+               const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw, uint32_t raw_len) {
+  InMsg& m = e->rx_msgs[i];
+  m = InMsg{};
   m.kind = kind; m.flags = flags; m.raw = raw; m.raw_len = raw_len;
-  if (kind == PCDN_KIND_DIRECT) { m.key = recipient; m.key_len = routed_key_len(e, recipient_len); }
-  else { m.topic_ids = topics; m.n_listed = m.n_topics = n_topics; }
-  return m;
+  if (kind == PCDN_KIND_DIRECT) {
+    m.key = recipient; m.key_len = routed_key_len(e, recipient_len);
+    m.stage_key = e->world_shards != e->shards.size();
+  } else {
+    m.topic_ids = topics; m.n_listed = m.n_topics = n_topics;
+  }
+  as_batch(e->rx_plan[i], m);
+}
+
+// MessageHookDef::on_message_received on the parsed message (def.rs:79-92).  Returns 0 = process,
+// 1 = skip, negative = error with its text in *why (the receive loop ends; the text may lie in hs.err).
+// The hook may shrink / rewrite the topic list (a private copy in hs.topics) and re-point the recipient.
+int run_hook(const pcdn_engine* e, uint32_t origin, const ParsedFrame& pf, const pcdn_frame& f, pcdn_engine::HookScratch& hs,
+             const uint8_t** f0, uint32_t* f0_len, const char** why) {
+  std::vector<uint8_t>& topic_copy = hs.topics;
+  pcdn_hook_message m{};
+  m.kind = (uint8_t)pf.kind; m.origin = (uint8_t)origin;
+  m.raw = f.raw; m.raw_len = f.raw_len; m.sender = f.sender; m.sender_len = f.sender_len;
+  const bool has_topics = pf.kind == PCDN_KIND_BROADCAST || pf.kind == PCDN_KIND_SUBSCRIBE || pf.kind == PCDN_KIND_UNSUBSCRIBE;
+  if (has_topics) {
+    if (pf.f0_len > 65535) { *why = "topic list too long"; return PCDN_EPARSE; }
+    topic_copy.assign(*f0, *f0 + pf.f0_len);
+    m.topics = topic_copy.data(); m.n_topics = (uint16_t)pf.f0_len;
+  } else if (pf.kind == PCDN_KIND_DIRECT) {
+    m.recipient = *f0; m.recipient_len = pf.f0_len;
+  }
+  const int r = e->hook[origin](e->hook_user[origin], &m);
+  if (r < 0) { hs.err = "hook failed: " + std::to_string(r); *why = hs.err.c_str(); return PCDN_EHOOK; }
+  if (r == PCDN_HOOK_SKIP) return 1;
+  if (has_topics) {
+    if (m.n_topics > topic_copy.size() || m.topics != topic_copy.data()) { *why = "hook returned an invalid topic list"; return PCDN_EHOOK; }
+    *f0 = topic_copy.data(); *f0_len = m.n_topics;
+  } else if (pf.kind == PCDN_KIND_DIRECT) {
+    if (m.recipient_len && !m.recipient) { *why = "hook returned a null recipient"; return PCDN_EHOOK; }
+    *f0 = m.recipient; *f0_len = m.recipient_len;
+  }
+  return 0;
+}
+
+// One iteration of user_receive_loop (origin 0, `sender` = the user's key) or broker_receive_loop
+// (origin 1, `sender` = the peer's identifier) up to the dispatch: frame `f` as entry `p` with message `m`.
+// It changes nothing in the engine, so phase A runs it on several threads.  A hook of f's origin runs in
+// it, with `hook` as its scratch, so hooked frames are classified by the scan, one at a time (phase A runs
+// only while no hook is set, and passes no scratch).
+void classify_frame(const pcdn_engine* e, const pcdn_frame& f, Entry& p, InMsg& m, pcdn_engine::HookScratch* hook) {
+  const uint32_t origin = f.origin ? 1 : 0;
+  m = InMsg{};
+  m.raw = f.raw; m.raw_len = f.raw_len; m.flags = origin ? MSGF_USERS_ONLY : 0;   // broker-origin messages go to users only
+  p.route = ROUTE_DONE; p.rc = 0; p.why = nullptr;
+  // device-parse engines without a hook for `origin`: a Direct or Broadcast frame is only tag-peeked and
+  // copied; k_parse does the rest
+  if ((e->cfg.flags & PCDN_FLAG_DEVICE_PARSE) && !e->hook[origin]) {
+    const int k = peek_kind_core(f.raw, f.raw_len);
+    if (k == PCDN_KIND_DIRECT || k == PCDN_KIND_BROADCAST) {
+      m.kind = (uint8_t)k;
+      m.flags |= MSGF_DEVPARSE | (k == PCDN_KIND_BROADCAST && !origin ? MSGF_PRUNE : 0);  // prune: user origin only (handler.rs:157 vs user/handler.rs:133)
+      return as_batch(p, m);
+    }
+  }
+  ParsedFrame pf;
+  if (!parse_frame(f.raw, f.raw_len, &pf)) { p.rc = PCDN_EPARSE; p.why = "failed to deserialize message"; return; }
+  const uint8_t* f0 = f.raw + pf.f0_off;   // field 0: the recipient or the wire topic list (a hook may replace it)
+  uint32_t f0_len = pf.f0_len;
+  if (e->hook[origin]) {
+    const int hr = run_hook(e, origin, pf, f, *hook, &f0, &f0_len, &p.why);
+    if (hr) { p.rc = hr < 0 ? hr : 0; return; }   // Ok(HookResult::SkipMessage) => continue
+  }
+  m.kind = (uint8_t)pf.kind;
+  if (pf.kind == PCDN_KIND_DIRECT) { m.key = f0; m.key_len = routed_key_len(e, f0_len); return as_batch(p, m); }
+  if (pf.kind != PCDN_KIND_BROADCAST) {
+    if (origin) { p.rc = 1; return; }
+    if (pf.kind != PCDN_KIND_SUBSCRIBE && pf.kind != PCDN_KIND_UNSUBSCRIBE) { p.rc = PCDN_EKIND; p.why = "invalid message received"; return; }
+  }
+  // A Broadcast or a user's Subscribe / Unsubscribe.  User-origin topic lists are pruned (Topic::prune,
+  // user/handler.rs:133), broker-origin ones kept verbatim (handler.rs:157).  The wire list may be of any
+  // length: what counts against a batch is the entries it adds (n_topics), which batch_limit judges.
+  m.wire_topics = f0; m.n_listed = f0_len; m.prune = !origin;
+  for (uint32_t t = 0; t < f0_len; t++) m.n_topics += !m.prune || topic_kept(f0, t, e->cfg.n_valid_topics) ? 1u : 0u;
+  if (m.n_topics == 0 && m.prune) { p.rc = PCDN_EPRUNE; p.why = "supplied no valid topics"; return; }
+  if (pf.kind == PCDN_KIND_BROADCAST) return as_batch(p, m);
+  p.route = (e->cfg.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) ? ROUTE_EVENT : ROUTE_STATE;
+  p.shape = MsgShape{m.kind, 0, 0, m.n_topics};
 }
 
 void slot_resize(Slot& s, const BatchFill& f) {
@@ -570,21 +638,30 @@ void slot_resize(Slot& s, const BatchFill& f) {
   s.aux_off.resize(f.msgs); s.aux_len.resize(f.msgs); s.bcast_index.resize(f.bcast); s.topics.resize(f.topics);
 }
 
-// Write message `mi` of slot `s`: its frame into the slot at arena offset `off` and its descriptor
-// entries (the arrays are sized already).  `aux_off`: a direct message's key offset in the arena (the
-// caller placed the key), a broadcast's first entry in s.topics; `bcast_pos`: a broadcast's place in
-// bcast_index.  It touches only what message mi owns, so threads may write distinct messages at once.
-void write_msg(Slot& s, uint32_t mi, size_t off, uint32_t aux_off, uint32_t bcast_pos, const InMsg& m, uint32_t n_valid) {
+// Write message `m`, placed by `p`, into slot `s`: its frame at p.arena_off, a staged recipient behind
+// the frame, and its descriptor entries (the arrays are sized already).  It touches only what this message
+// owns, so threads may write distinct messages at once.
+void write_msg(Slot& s, const Entry& p, const InMsg& m, uint32_t n_valid) {
+  const size_t off = p.arena_off, slot = align_up(4 + (size_t)m.raw_len, 16);
+  const uint32_t mi = p.msg_idx;
   uint8_t* dst = s.h_arena + off;
   std::memset(dst, 0, 4);
   if (m.raw_len) std::memcpy(dst + 4, m.raw, m.raw_len);
-  std::memset(dst + 4 + m.raw_len, 0, align_up(4 + (size_t)m.raw_len, 16) - 4 - m.raw_len);
+  std::memset(dst + 4 + m.raw_len, 0, slot - 4 - m.raw_len);
   s.kind[mi] = m.kind; s.flags[mi] = m.flags; s.slot_off16[mi] = (uint32_t)(off / 16); s.raw_len[mi] = m.raw_len;
-  s.aux_off[mi] = aux_off;
-  if (m.kind == PCDN_KIND_DIRECT) { s.aux_len[mi] = m.key_len; return; }
+  if (m.kind == PCDN_KIND_DIRECT) {
+    if (m.stage_key) {
+      if (m.key_len) std::memcpy(dst + slot, m.key, m.key_len);
+      std::memset(dst + slot + m.key_len, 0, p.shape.key_bytes - m.key_len);
+    }
+    s.aux_off[mi] = (uint32_t)(m.stage_key ? off + slot : off + 4 + (size_t)(m.key - m.raw));
+    s.aux_len[mi] = m.key_len;
+    return;
+  }
+  s.aux_off[mi] = p.topic_off;
   s.aux_len[mi] = m.n_topics;
-  s.bcast_index[bcast_pos] = mi;
-  for (uint32_t t = 0, k = aux_off; t < m.n_listed; t++) {
+  s.bcast_index[p.bcast_pos] = mi;
+  for (uint32_t t = 0, k = p.topic_off; t < m.n_listed; t++) {
     if (m.topic_ids) s.topics[k++] = m.topic_ids[t];
     else if (!m.prune || topic_kept(m.wire_topics, t, n_valid)) s.topics[k++] = m.wire_topics[t];
   }
@@ -596,41 +673,142 @@ void slot_commit(pcdn_engine* e, Slot& s, const BatchFill& f, bool devparse) {
   s.ingress_bytes += f.ingress; e->inflight_bytes += f.ingress; e->stats.bytes_in += f.ingress;
 }
 
-// append one message to the open batch (launching a full batch first)
-int append_msg(pcdn_engine* e, const InMsg& m) {
-  if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
-  if (m.kind != PCDN_KIND_BROADCAST && m.kind != PCDN_KIND_DIRECT) return fail(PCDN_EINVAL, "kind must be broadcast or direct");
-  const bool direct = m.kind == PCDN_KIND_DIRECT;
-  MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(m.key_len, 16) : 0u, m.n_topics};  // key staged: the worst case
-  if (const char* why = msg_invalid(e, m.raw_len)) return fail(PCDN_EINVAL, why);
-  if (const char* lim = batch_limit(e, BatchFill{}, shape)) return fail(PCDN_ENOSPC, std::string("message does not fit an empty batch: ") + lim);
-  if (!pool_admits(e, m.raw_len)) return fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
-  int rc = acquire_open_slot(e);
-  if (!rc && batch_limit(e, fill_of(e->slots[e->open_slot]), shape) && !(rc = flush_open(e, nullptr))) rc = acquire_open_slot(e);
-  if (rc) return rc;
-  Slot& s = e->slots[e->open_slot];
-  BatchFill f = fill_of(s);
-  const size_t off = f.bytes;  // 16-byte aligned
-  uint32_t aux_off = (uint32_t)f.topics;
-  if (direct) {
-    // recipient key: read it in place when it lies inside the frame at a 4-byte aligned offset
-    // (multi-process groups always stage it beside the frame: the layout must not depend on how a
-    // process happens to hold the bytes)
-    if (m.key_len && m.key >= m.raw && m.key + m.key_len <= m.raw + m.raw_len &&
-        ((off + 4 + (size_t)(m.key - m.raw)) & 3) == 0 && e->world_shards == e->shards.size()) {
-      aux_off = (uint32_t)(off + 4 + (size_t)(m.key - m.raw));
-      shape.key_bytes = 0;
-    } else {
-      aux_off = (uint32_t)(off + align_up(4 + (size_t)m.raw_len, 16));
-      if (m.key_len) std::memcpy(s.h_arena + aux_off, m.key, m.key_len);
-      std::memset(s.h_arena + aux_off + m.key_len, 0, shape.key_bytes - m.key_len);
-    }
+template <class F>
+void parallel_for(uint32_t n, uint32_t nthreads, F f) {
+  if (n < 2048 || nthreads <= 1) { f(0u, n); return; }
+  std::vector<std::thread> th;
+  const uint32_t per = (n + nthreads - 1) / nthreads;
+  for (uint32_t t = 1; t < nthreads; t++) {
+    const uint32_t lo = t * per, hi = std::min(n, lo + per);
+    if (lo < hi) th.emplace_back([=] { f(lo, hi); });
   }
-  f.add(shape);
-  slot_resize(s, f);
-  write_msg(s, f.msgs - 1, off, aux_off, f.bcast - 1, m, e->cfg.n_valid_topics);
-  slot_commit(e, s, f, (m.flags & MSGF_DEVPARSE) != 0);
-  return 0;
+  f(0u, std::min(n, per));
+  for (auto& x : th) x.join();
+}
+
+uint32_t ingest_threads() {
+  static uint32_t n = [] {
+    if (const char* e = std::getenv("PCDN_INGEST_THREADS")) return (uint32_t)std::max(1, atoi(e));
+    return std::min(16u, std::max(1u, std::thread::hardware_concurrency()));
+  }();
+  return n;
+}
+
+// The placement scan: the scratch entries [0, n) in order, on the calling thread (each classified here
+// first when `classify` is set; `frames`: the frames behind them, null for API messages).  An entry is
+// placed in the open batch (launching a full one first), recorded as an event of it, applied through
+// sub_change, or only reported.  Its result goes to Entry::rc and rc_out[i], a failure's text to
+// pcdn_last_error.  The placed messages of a run are written by index (phase B, on several threads for
+// long runs) before the batch is launched or anything else changes it.  Returns the number of entries
+// consumed (a capacity condition, a CUDA error or a host-only engine stops early) or the code when not
+// even the first one was.
+int place_entries(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t* rc_out, bool classify) {
+  Entry* const plan = e->rx_plan.get();
+  InMsg* const msgs = e->rx_msgs.get();
+  const uint32_t n_valid = e->cfg.n_valid_topics;
+  BatchFill fill;   // while `open`: the open batch, holding the messages placed by entries [run, i)
+  bool open = false, devparse = false;
+  uint32_t run = 0;
+  auto end_run = [&](uint32_t end) {
+    if (!open) return;
+    Slot& s = e->slots[e->open_slot];
+    slot_resize(s, fill);
+    parallel_for(end - run, ingest_threads(), [&](uint32_t lo, uint32_t hi) {
+      for (uint32_t q = run + lo; q < run + hi; q++)
+        if (plan[q].route == ROUTE_BATCH) write_msg(s, plan[q], msgs[q], n_valid);
+    });
+    slot_commit(e, s, fill, devparse);
+    open = devparse = false;
+  };
+  for (uint32_t i = 0; i < n; i++) {
+    Entry& p = plan[i];
+    if (classify) classify_frame(e, frames[i], p, msgs[i], &e->rx_hook);
+    int rc = p.rc;
+    if (p.route == ROUTE_BATCH) {
+      const char* why;
+      if (!e->has_device) rc = fail(PCDN_ENODEV, "host-only engine cannot route messages");
+      else if ((why = msg_invalid(e, p.shape.raw_len))) rc = fail(PCDN_EINVAL, why);
+      else if ((why = batch_limit(e, BatchFill{}, p.shape))) rc = fail(PCDN_ENOSPC, std::string("message does not fit an empty batch: ") + why);
+      else for (bool launched = false;; launched = true) {   // the open batch, else a new one behind it
+        if (!open) {
+          if ((rc = acquire_open_slot(e))) break;
+          fill = fill_of(e->slots[e->open_slot]);
+          open = true; run = i;
+        }
+        if (!batch_limit(e, fill, p.shape) && pool_admits(e, fill.ingress + p.shape.raw_len)) {
+          p.msg_idx = fill.msgs; p.arena_off = fill.bytes; p.bcast_pos = fill.bcast; p.topic_off = (uint32_t)fill.topics;
+          fill.add(p.shape);
+          devparse |= p.devparse;
+          break;
+        }
+        // Only an exhausted memory pool refuses an empty batch.  Its permits come back when batches are
+        // released, so the open batch is launched first: then draining a batch and calling again makes progress.
+        if (launched) { rc = fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first"); break; }
+        end_run(i);
+        if ((rc = flush_open(e, nullptr))) break;
+      }
+      if (rc) p.route = ROUTE_DONE;   // (phase B skips it)
+    } else if (p.route != ROUTE_DONE) {   // a user's Subscribe / Unsubscribe
+      const InMsg& m = msgs[i];
+      e->rx_topics.resize(m.n_listed);
+      const uint32_t nt = prune_topics(m.wire_topics, m.n_listed, n_valid, e->rx_topics.data());
+      const SubOp op = m.kind == PCDN_KIND_SUBSCRIBE ? SUB_USER : UNSUB_USER;
+      const std::string who((const char*)frames[i].sender, frames[i].sender_len);
+      rc = 1;
+      if (p.route == ROUTE_EVENT && open) {   // an event at its place among the messages: the run goes on
+        rc = record_event(e, fill, op, who, e->rx_topics.data(), nt);
+        fill.ev_topics = e->slots[e->open_slot].ev_topics.size();
+        if (rc < 0) fail(rc, "topic id out of range");
+      }
+      if (rc == 1) {
+        end_run(i);
+        rc = sub_change(e, op, who, e->rx_topics.data(), nt);
+      }
+    } else if (rc < 0) {
+      fail(rc, p.why);
+    }
+    p.rc = rc;
+    if (rc_out) rc_out[i] = rc;
+    if (rc == PCDN_EAGAIN || rc == PCDN_ECUDA || rc == PCDN_ENODEV) {
+      end_run(i);
+      return i ? (int)i : rc;
+    }
+    if (classify) end_run(i + 1);   // (the next classification reuses the hook's scratch)
+  }
+  end_run(n);
+  return (int)n;
+}
+
+// one message of pcdn_handle_*_message through the placement scan
+int handle_msg(pcdn_engine* e, uint8_t kind, uint8_t flags, const uint16_t* topics, uint32_t n_topics,
+               const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw, uint32_t raw_len) {
+  e->rx_reserve(1);
+  api_entry(e, 0, kind, flags, topics, n_topics, recipient, recipient_len, raw, raw_len);
+  place_entries(e, nullptr, 1, nullptr, false);
+  return e->rx_plan[0].rc;
+}
+
+// pcdn_receive_frames: phase A classifies every frame (on several threads for large calls), unless a hook
+// is set: the scan then classifies each frame when it comes to it, so that the hook sees the frames in
+// order and only those the call consumes
+int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t* rc_out) {
+  e->rx_reserve(n);
+  const bool hooked = e->hook[0] || e->hook[1];
+  if (!hooked)
+    parallel_for(n, ingest_threads(), [&](uint32_t lo, uint32_t hi) {
+      for (uint32_t i = lo; i < hi; i++) classify_frame(e, frames[i], e->rx_plan[i], e->rx_msgs[i], nullptr);
+    });
+  const int done = place_entries(e, frames, n, rc_out, hooked);
+  e->rx_release();
+  return done;
+}
+
+// one frame through pcdn_receive_frames: what it returns for that frame
+int receive_one(pcdn_engine* e, uint32_t origin, const uint8_t* sender, uint32_t sender_len, const uint8_t* raw, uint32_t raw_len) {
+  const pcdn_frame f{sender, sender_len, origin, raw, raw_len, 0};
+  int32_t rc = 0;
+  receive_frames_locked(e, &f, 1, &rc);
+  return rc;
 }
 
 }  // namespace
@@ -1183,276 +1361,30 @@ int pcdn_handle_broadcast_message(pcdn_engine* e, const uint16_t* topics, uint32
                                   uint32_t raw_len, int to_users_only) {
   GUARD_BEGIN
   LOCK;
-  return append_msg(e, api_msg(e, PCDN_KIND_BROADCAST, to_users_only ? PCDN_TO_USERS_ONLY : 0, topics, n_topics, nullptr, 0, raw, raw_len));
+  return handle_msg(e, PCDN_KIND_BROADCAST, to_users_only ? PCDN_TO_USERS_ONLY : 0, topics, n_topics, nullptr, 0, raw, raw_len);
   GUARD_END
 }
 int pcdn_handle_direct_message(pcdn_engine* e, const uint8_t* recipient, uint32_t recipient_len, const uint8_t* raw,
                                uint32_t raw_len, int to_user_only) {
   GUARD_BEGIN
   LOCK;
-  return append_msg(e, api_msg(e, PCDN_KIND_DIRECT, to_user_only ? PCDN_TO_USERS_ONLY : 0, nullptr, 0, recipient, recipient_len, raw, raw_len));
+  return handle_msg(e, PCDN_KIND_DIRECT, to_user_only ? PCDN_TO_USERS_ONLY : 0, nullptr, 0, recipient, recipient_len, raw, raw_len);
   GUARD_END
-}
-
-// ---- frames to messages: user_receive_loop / broker_receive_loop (user/handler.rs, broker/handler.rs) ----
-// Device-parse engines without a hook for `origin`: a Direct or Broadcast frame is only tag-peeked
-// and copied; k_parse does the rest.  false: the frame takes the host parse.
-static bool devparse_msg(const pcdn_engine* e, uint32_t origin, const uint8_t* raw, uint32_t raw_len, InMsg* m) {
-  if (!(e->cfg.flags & PCDN_FLAG_DEVICE_PARSE) || e->hook[origin]) return false;
-  const int k = peek_kind_core(raw, raw_len);
-  if (k != PCDN_KIND_DIRECT && k != PCDN_KIND_BROADCAST) return false;
-  *m = InMsg{};
-  m->kind = (uint8_t)k; m->raw = raw; m->raw_len = raw_len;
-  m->flags = MSGF_DEVPARSE | (origin ? MSGF_USERS_ONLY : 0) | (k == PCDN_KIND_BROADCAST && !origin ? MSGF_PRUNE : 0);  // prune: user origin only (handler.rs:157 vs user/handler.rs:133)
-  return true;
-}
-
-// A parsed Direct or Broadcast frame as a message.  `f0` is its field 0 (the recipient or the wire topic
-// list; a hook may have replaced it).  Broker-origin messages go to users only; user-origin topic lists
-// are pruned (Topic::prune, user/handler.rs:133), broker-origin ones kept verbatim (handler.rs:157).
-// The wire list may be of any length: what counts against a batch is the entries it adds (n_topics),
-// which the admission rule (batch_limit) judges.  0, or an error code and *why.
-static int parsed_msg(const pcdn_engine* e, uint32_t origin, int kind, const uint8_t* raw, uint32_t raw_len,
-                      const uint8_t* f0, uint32_t f0_len, InMsg* m, const char** why) {
-  *m = InMsg{};
-  m->kind = (uint8_t)kind; m->raw = raw; m->raw_len = raw_len; m->flags = origin ? MSGF_USERS_ONLY : 0;
-  if (kind == PCDN_KIND_DIRECT) { m->key = f0; m->key_len = routed_key_len(e, f0_len); return 0; }
-  m->wire_topics = f0; m->n_listed = f0_len; m->prune = !origin;
-  for (uint32_t t = 0; t < f0_len; t++) m->n_topics += !m->prune || topic_kept(f0, t, e->cfg.n_valid_topics) ? 1u : 0u;
-  if (m->n_topics == 0 && m->prune) { *why = "supplied no valid topics"; return PCDN_EPRUNE; }
-  return 0;
-}
-
-// MessageHookDef::on_message_received on the parsed message (def.rs:79-92).  Returns 0 = process,
-// 1 = skip, negative = error (the receive loop ends).  The hook may shrink / rewrite the topic list
-// (a private copy) and re-point the recipient.
-static int run_hook(pcdn_engine* e, int origin, const ParsedFrame& pf, const uint8_t* sender, uint32_t sender_len,
-                    const uint8_t* raw, uint32_t raw_len, std::vector<uint8_t>& topic_copy, const uint8_t** f0, uint32_t* f0_len) {
-  *f0 = raw + pf.f0_off; *f0_len = pf.f0_len;
-  if (!e->hook[origin]) return 0;
-  pcdn_hook_message m{};
-  m.kind = (uint8_t)pf.kind; m.origin = (uint8_t)origin;
-  m.raw = raw; m.raw_len = raw_len; m.sender = sender; m.sender_len = sender_len;
-  const bool has_topics = pf.kind == PCDN_KIND_BROADCAST || pf.kind == PCDN_KIND_SUBSCRIBE || pf.kind == PCDN_KIND_UNSUBSCRIBE;
-  if (has_topics) {
-    if (pf.f0_len > 65535) return fail(PCDN_EPARSE, "topic list too long");
-    topic_copy.assign(raw + pf.f0_off, raw + pf.f0_off + pf.f0_len);
-    m.topics = topic_copy.data(); m.n_topics = (uint16_t)pf.f0_len;
-  } else if (pf.kind == PCDN_KIND_DIRECT) {
-    m.recipient = raw + pf.f0_off; m.recipient_len = pf.f0_len;
-  }
-  const int r = e->hook[origin](e->hook_user[origin], &m);
-  if (r < 0) return fail(PCDN_EHOOK, "hook failed: " + std::to_string(r));
-  if (r == PCDN_HOOK_SKIP) return 1;
-  if (has_topics) {
-    if (m.n_topics > topic_copy.size() || m.topics != topic_copy.data()) return fail(PCDN_EHOOK, "hook returned an invalid topic list");
-    *f0 = topic_copy.data(); *f0_len = m.n_topics;
-  } else if (pf.kind == PCDN_KIND_DIRECT) {
-    if (m.recipient_len && !m.recipient) return fail(PCDN_EHOOK, "hook returned a null recipient");
-    *f0 = m.recipient; *f0_len = m.recipient_len;
-  }
-  return 0;
-}
-
-// One iteration of user_receive_loop (origin 0, `sender` = the user's key) or broker_receive_loop
-// (origin 1, `sender` = the peer's identifier).  A broker-origin frame of another kind returns 1.
-static int receive_locked(pcdn_engine* e, uint32_t origin, const uint8_t* sender, uint32_t sender_len, const uint8_t* raw, uint32_t raw_len) {
-  InMsg m;
-  if (devparse_msg(e, origin, raw, raw_len, &m)) return append_msg(e, m);
-  ParsedFrame pf;
-  if (!parse_frame(raw, raw_len, &pf)) return fail(PCDN_EPARSE, "failed to deserialize message");
-  std::vector<uint8_t> hooked_topics;
-  const uint8_t* f0; uint32_t f0_len;
-  int hr = run_hook(e, (int)origin, pf, sender, sender_len, raw, raw_len, hooked_topics, &f0, &f0_len);
-  if (hr < 0) return hr;
-  if (hr == 1) return 0;  // Ok(HookResult::SkipMessage) => continue
-  if (pf.kind == PCDN_KIND_DIRECT || pf.kind == PCDN_KIND_BROADCAST) {
-    const char* why = "";
-    const int rc = parsed_msg(e, origin, pf.kind, raw, raw_len, f0, f0_len, &m, &why);
-    return rc ? fail(rc, why) : append_msg(e, m);
-  }
-  if (origin) return 1;
-  if (pf.kind != PCDN_KIND_SUBSCRIBE && pf.kind != PCDN_KIND_UNSUBSCRIBE) return fail(PCDN_EKIND, "invalid message received");
-  std::vector<uint16_t> topics(f0_len);  // the wire list may be of any length, as in the reference
-  uint32_t n = prune_topics(f0, f0_len, e->cfg.n_valid_topics, topics.data());
-  if (n == 0) return fail(PCDN_EPRUNE, "supplied no valid topics");
-  return sub_change(e, pf.kind == PCDN_KIND_SUBSCRIBE ? SUB_USER : UNSUB_USER, std::string((const char*)sender, sender_len), topics.data(), n);
 }
 
 int pcdn_user_receive(pcdn_engine* e, const uint8_t* sender_key, uint32_t key_len, const uint8_t* raw, uint32_t raw_len) {
   GUARD_BEGIN
   LOCK;
-  return receive_locked(e, 0, sender_key, key_len, raw, raw_len);
+  return receive_one(e, 0, sender_key, key_len, raw, raw_len);
   GUARD_END
 }
 
 int pcdn_broker_receive(pcdn_engine* e, const char* identifier, const uint8_t* raw, uint32_t raw_len) {
   GUARD_BEGIN
   LOCK;
-  return receive_locked(e, 1, (const uint8_t*)identifier, identifier ? (uint32_t)std::strlen(identifier) : 0, raw, raw_len);
+  return receive_one(e, 1, (const uint8_t*)identifier, identifier ? (uint32_t)std::strlen(identifier) : 0, raw, raw_len);
   GUARD_END
 }
-
-// ---- multi-threaded ingest of many frames -----------------------------------------------------
-extern "C++" {
-namespace {
-
-enum FrameRoute : int8_t { ROUTE_SEQUENTIAL, ROUTE_FAILED, ROUTE_BATCH, ROUTE_EVENT };
-// what the serial placement scan reads and writes per frame (kept small: the scan streams through it)
-struct FramePlan {
-  // ROUTE_SEQUENTIAL: the frame goes through user/broker_receive_locked (state change, other kinds, a
-  // message no batch takes, which reports its error there); ROUTE_FAILED: protocol error `rc`;
-  // ROUTE_EVENT (PCDN_FLAG_INBATCH_SUBSCRIBE): a user's Subscribe / Unsubscribe, recorded by the scan
-  FrameRoute route;
-  int32_t rc;
-  MsgShape shape;
-  uint32_t msg_idx, bcast_pos, topic_off;
-  uint64_t arena_off;
-};
-
-template <class F>
-void parallel_for(uint32_t n, uint32_t nthreads, F f) {
-  if (n < 2048 || nthreads <= 1) { f(0u, n); return; }
-  std::vector<std::thread> th;
-  const uint32_t per = (n + nthreads - 1) / nthreads;
-  for (uint32_t t = 1; t < nthreads; t++) {
-    const uint32_t lo = t * per, hi = std::min(n, lo + per);
-    if (lo < hi) th.emplace_back([=] { f(lo, hi); });
-  }
-  f(0u, std::min(n, per));
-  for (auto& x : th) x.join();
-}
-
-uint32_t ingest_threads() {
-  static uint32_t n = [] {
-    if (const char* e = std::getenv("PCDN_INGEST_THREADS")) return (uint32_t)std::max(1, atoi(e));
-    return std::min(16u, std::max(1u, std::thread::hardware_concurrency()));
-  }();
-  return n;
-}
-
-// One receive-loop iteration per frame, in order; returns the number of frames consumed (a capacity
-// condition — no free batch slot, memory pool exhausted — stops early) or a negative error when
-// nothing could be consumed.  Large calls run in three phases per run of routable frames:
-//   A (parallel)  parse (host mode) or tag peek (device-parse mode) of every frame
-//   scan (serial) a few integer adds per frame: placement in the open batch, capacity, ordering
-//   B (parallel)  copy of the raw bytes into the pinned arena + descriptor fill by index
-// Frames that change state (Subscribe/Unsubscribe) or need the exact synchronous error path end a
-// run and go through user_receive_locked / broker_receive_locked, so R12 ordering is untouched.
-// PCDN_FLAG_INBATCH_SUBSCRIBE: a user's Subscribe / Unsubscribe is parsed and pruned in phase A and
-// becomes an event of the open batch in the scan (at its place among the messages); it ends the run
-// only when the batch cannot take the event.
-int receive_frames_locked(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t* rc_out) {
-  const pcdn_config& c = e->cfg;
-  const uint32_t T = ingest_threads();
-  const bool inbatch = (c.flags & PCDN_FLAG_INBATCH_SUBSCRIBE) != 0;
-  // a hook sees every parsed message, in order
-  const bool threaded = n >= 2048 && T > 1 && e->has_device && !e->hook[0] && !e->hook[1];
-  // phase A writes every entry the later phases read
-  std::unique_ptr<FramePlan[]> plan(threaded ? new FramePlan[n] : nullptr);
-  std::unique_ptr<InMsg[]> msgs(threaded ? new InMsg[n] : nullptr);
-  // ---- phase A
-  if (threaded) parallel_for(n, T, [&](uint32_t lo, uint32_t hi) {
-    for (uint32_t i = lo; i < hi; i++) {
-      const pcdn_frame& f = frames[i];
-      FramePlan& p = plan[i];
-      InMsg& m = msgs[i];
-      const uint32_t origin = f.origin ? 1 : 0;
-      p.route = ROUTE_SEQUENTIAL; p.rc = 0;
-      if (!devparse_msg(e, origin, f.raw, f.raw_len, &m)) {
-        const bool dp = (c.flags & PCDN_FLAG_DEVICE_PARSE) != 0, ev = inbatch && !origin;
-        if (dp && !ev) continue;
-        ParsedFrame pf;
-        const char* why;
-        if (!parse_frame(f.raw, f.raw_len, &pf)) {
-          if (!dp) { p.route = ROUTE_FAILED; p.rc = PCDN_EPARSE; }
-          continue;
-        }
-        if (ev && (pf.kind == PCDN_KIND_SUBSCRIBE || pf.kind == PCDN_KIND_UNSUBSCRIBE)) {
-          m = InMsg{};
-          m.kind = (uint8_t)pf.kind; m.wire_topics = f.raw + pf.f0_off; m.n_listed = pf.f0_len;
-          for (uint32_t t = 0; t < pf.f0_len; t++) m.n_topics += topic_kept(m.wire_topics, t, c.n_valid_topics) ? 1u : 0u;
-          if (m.n_topics) p.route = ROUTE_EVENT;
-          else { p.route = ROUTE_FAILED; p.rc = PCDN_EPRUNE; }
-          continue;
-        }
-        if (dp || (pf.kind != PCDN_KIND_DIRECT && pf.kind != PCDN_KIND_BROADCAST)) continue;
-        p.rc = parsed_msg(e, origin, pf.kind, f.raw, f.raw_len, f.raw + pf.f0_off, pf.f0_len, &m, &why);
-        if (p.rc) { p.route = ROUTE_FAILED; continue; }
-      }
-      p.shape = MsgShape{m.kind, m.raw_len, 0, m.n_topics};   // the parsed recipient is read in place
-      if (!msg_invalid(e, f.raw_len) && !batch_limit(e, BatchFill{}, p.shape)) p.route = ROUTE_BATCH;
-    }
-  });
-  uint32_t i = 0;
-  while (i < n) {
-    if (!threaded || plan[i].route == ROUTE_SEQUENTIAL) {
-      const pcdn_frame& f = frames[i];
-      int rc = receive_locked(e, f.origin ? 1 : 0, f.sender, f.sender_len, f.raw, f.raw_len);
-      if (rc_out) rc_out[i] = rc;
-      if (rc == PCDN_EAGAIN || rc == PCDN_ECUDA || rc == PCDN_ENODEV) return i ? (int)i : rc;
-      i++;
-      continue;
-    }
-    if (plan[i].route == ROUTE_FAILED) { if (rc_out) rc_out[i] = plan[i].rc; i++; continue; }
-    // ---- a run of routable frames starting at i: placement scan
-    int rc = acquire_open_slot(e);
-    if (rc) return i ? (int)i : rc;
-    Slot& s = e->slots[e->open_slot];
-    BatchFill fill = fill_of(s);
-    uint32_t j = i;
-    bool full = false;
-    for (; j < n; j++) {
-      FramePlan& p = plan[j];
-      if (p.route == ROUTE_FAILED) continue;
-      if (p.route == ROUTE_SEQUENTIAL) break;
-      if (p.route == ROUTE_EVENT) {
-        const InMsg& m = msgs[j];
-        if (!event_fits(e, fill, m.n_topics)) { p.route = ROUTE_SEQUENTIAL; break; }   // launch, then the change
-        std::vector<uint16_t> topics(m.n_listed);
-        const uint32_t nt = prune_topics(m.wire_topics, m.n_listed, c.n_valid_topics, topics.data());
-        const pcdn_frame& f = frames[j];
-        p.rc = record_event(e, fill.msgs, m.kind == PCDN_KIND_SUBSCRIBE ? SUB_USER : UNSUB_USER,
-                            std::string((const char*)f.sender, f.sender_len), topics.data(), nt);
-        if (p.rc) fail(p.rc, "topic id out of range");
-        fill.ev_topics = s.ev_topics.size();
-        continue;
-      }
-      if (batch_limit(e, fill, p.shape) || !pool_admits(e, fill.ingress + p.shape.raw_len)) { full = true; break; }
-      p.msg_idx = fill.msgs; p.arena_off = fill.bytes; p.bcast_pos = fill.bcast; p.topic_off = (uint32_t)fill.topics;
-      fill.add(p.shape);
-    }
-    if (j == i && plan[i].route == ROUTE_SEQUENTIAL) continue;   // an event the open batch cannot take
-    if (j == i) {  // nothing fits: the open batch is full (or the pool is) — launch it and retry, or give up
-      if (s.kind.empty()) return i ? (int)i : fail(PCDN_EAGAIN, "global memory pool exhausted: release a batch first");
-      if ((rc = flush_open(e, nullptr))) return i ? (int)i : rc;
-      continue;
-    }
-    // ---- phase B: raw bytes + descriptors by index
-    slot_resize(s, fill);
-    parallel_for(j - i, T, [&](uint32_t lo, uint32_t hi) {
-      for (uint32_t q = i + lo; q < i + hi; q++) {
-        const FramePlan& p = plan[q];
-        const InMsg& m = msgs[q];
-        if (p.route != ROUTE_BATCH) continue;
-        const uint32_t aux_off = m.kind == PCDN_KIND_BROADCAST ? p.topic_off
-                                 : m.key ? (uint32_t)(p.arena_off + 4 + (size_t)(m.key - m.raw)) : 0;  // recipient read in place (word aligned)
-        write_msg(s, p.msg_idx, p.arena_off, aux_off, p.bcast_pos, m, c.n_valid_topics);
-      }
-    });
-    if (rc_out)
-      for (uint32_t q = i; q < j; q++) rc_out[q] = plan[q].rc;
-    slot_commit(e, s, fill, (c.flags & PCDN_FLAG_DEVICE_PARSE) != 0);
-    i = j;
-    if (full) {
-      if ((rc = flush_open(e, nullptr))) return (int)i;
-    }
-  }
-  return (int)n;
-}
-
-}  // namespace
-}  // extern "C++"
 
 int pcdn_set_message_hook(pcdn_engine* e, int origin, pcdn_message_hook cb, void* user) {
   GUARD_BEGIN
@@ -1520,13 +1452,17 @@ int pcdn_submit(pcdn_engine* e, const pcdn_msg* msgs, uint32_t n, uint64_t* batc
   if (rc) return rc;
   if (n == 0) return 0;
   if ((rc = acquire_open_slot(e))) return rc;  // PCDN_EAGAIN: nothing staged
+  e->rx_reserve(n);
   for (uint32_t i = 0; i < n; i++) {
     const pcdn_msg& m = msgs[i];
-    uint64_t before = e->next_batch_id;
-    rc = append_msg(e, api_msg(e, m.kind, m.flags, m.topics, m.n_topics, m.recipient, m.recipient_len, m.raw, m.raw_len));
-    if (rc == 0 && e->next_batch_id != before) rc = fail(PCDN_ENOSPC, "batch exceeded a per-batch capacity and was split");
-    if (rc) { abandon_open(e); return rc; }  // unreachable after validation; never leave a half batch open
+    api_entry(e, i, m.kind, m.flags, m.topics, m.n_topics, m.recipient, m.recipient_len, m.raw, m.raw_len);
   }
+  const uint64_t before = e->next_batch_id;
+  place_entries(e, nullptr, n, nullptr, false);
+  for (uint32_t i = 0; i < n && !rc; i++) rc = e->rx_plan[i].rc;
+  e->rx_release();
+  if (rc == 0 && e->next_batch_id != before) rc = fail(PCDN_ENOSPC, "batch exceeded a per-batch capacity and was split");
+  if (rc) { abandon_open(e); return rc; }  // unreachable after validation; never leave a half batch open
   return flush_open(e, batch_id);
   GUARD_END
 }

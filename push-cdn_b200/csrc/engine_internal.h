@@ -153,6 +153,46 @@ struct Slot {
   std::vector<pcdn_conn> merged_overflow;
 };
 
+// One message on its way into a batch (an aggregate: InMsg{} is the empty message).
+struct InMsg {
+  uint8_t kind, flags;
+  bool prune;                        // broadcast: apply Topic::prune to the wire topic list
+  bool stage_key;                    // direct: the recipient is copied beside the frame, not read in place
+  uint32_t raw_len, key_len;         // key_len: direct message's recipient length (routed_key_len)
+  uint32_t n_listed, n_topics;       // broadcast: entries of the topic list below, entries it adds to the batch
+  const uint8_t* raw;
+  const uint8_t* key;                // direct: the recipient
+  const uint16_t* topic_ids;         // broadcast: the topic ids (API calls), or null and
+  const uint8_t* wire_topics;        // a frame's wire topic list, pruned or verbatim
+};
+
+// What one message adds to a batch: a 16-byte frame slot (4-byte length hole, raw bytes, zero pad),
+// `key_bytes` of recipient key staged beside it (0 when the key is read in place) and topic entries.
+struct MsgShape {
+  uint8_t kind;
+  uint32_t raw_len, key_bytes, n_topics;
+  size_t bytes() const { return align_up(4 + (size_t)raw_len, 16) + key_bytes; }
+};
+
+// What the placement scan does with a classified frame or API message:
+//   BATCH  place `InMsg` in the open batch;
+//   EVENT  (PCDN_FLAG_INBATCH_SUBSCRIBE) a user's Subscribe / Unsubscribe, an event of the open batch;
+//   STATE  a Subscribe / Unsubscribe through sub_change (the open batch is launched first, R12);
+//   DONE   nothing to place: the result is `rc` (a protocol error with its text `why`, a hook's Skip,
+//          1 for a broker frame of another kind).
+enum Route : int8_t { ROUTE_BATCH, ROUTE_EVENT, ROUTE_STATE, ROUTE_DONE };
+// what the serial placement scan reads and writes per entry (kept small: the scan streams through it;
+// the InMsg of entry i lies beside it)
+struct Entry {
+  Route route;
+  bool devparse;      // BATCH: the message carries MSGF_DEVPARSE
+  int32_t rc;         // the entry's result, once the scan has handled it
+  const char* why;    // DONE with rc < 0: the pcdn_last_error text
+  MsgShape shape;     // BATCH; EVENT / STATE: shape.n_topics is the pruned topic count
+  uint32_t msg_idx, bcast_pos, topic_off;   // BATCH: its place in the open batch, set by the scan
+  uint64_t arena_off;
+};
+
 // make `dev` current for the calling thread for the lifetime of the guard (cheap when it already is)
 struct DeviceGuard {
   int prev = -1; bool switched = false;
@@ -194,6 +234,24 @@ struct pcdn_engine {
   void* hook_user[2] = {nullptr, nullptr};
   uint64_t inflight_bytes = 0;  // Limiter analogue: accepted frame bytes whose batch is not released yet
   pcdn_stats stats{};
+  // receive / handle / submit scratch: the classified entries of a call and their messages.  Left
+  // uninitialised (a large call pays no clearing); kept for the next call while they hold at most kRxKeep
+  // entries, so small calls allocate nothing, and freed at the end of a larger call.
+  static constexpr uint32_t kRxKeep = 1u << 16;
+  std::unique_ptr<Entry[]> rx_plan;
+  std::unique_ptr<InMsg[]> rx_msgs;
+  uint32_t rx_cap = 0;
+  void rx_reserve(uint32_t n) {
+    if (n > rx_cap) { rx_plan.reset(new Entry[n]); rx_msgs.reset(new InMsg[n]); rx_cap = n; }
+  }
+  void rx_release() {
+    if (rx_cap > kRxKeep) { rx_plan.reset(); rx_msgs.reset(); rx_cap = 0; }
+  }
+  std::vector<uint16_t> rx_topics;   // a Subscribe's pruned topics
+  struct HookScratch {               // a hooked frame's private topic list, and the text of a hook's error
+    std::vector<uint8_t> topics;
+    std::string err;
+  } rx_hook;
   // buffers behind pcdn_get_*_sync
   std::vector<UserSyncEntry> sync_users;
   std::vector<pcdn_user_sync_entry> sync_users_c;

@@ -100,7 +100,7 @@ def test_msg_status_codes(pcdn, staged):
 @pytest.mark.parametrize("flags", [0, 1], ids=["host-parse", "device-parse"])
 def test_large_call_takes_the_threaded_path(pcdn, flags):
     """>= 2048 frames in one pcdn_receive_frames call: parallel parse/peek + parallel copy, with
-    Subscribe/Unsubscribe frames (state changes, sequential path), malformed frames and batch
+    Subscribe/Unsubscribe frames (state changes that launch the open batch), malformed frames and batch
     capacity boundaries in the middle — order and outcomes must equal the one-at-a-time oracle"""
     rng = random.Random(99)
     w = World(pcdn, n_valid_topics=10, flags=flags, ring_bytes_per_conn=1 << 20, max_batch_msgs=1500, max_batch_bcast=512,

@@ -392,6 +392,7 @@ def test_global_memory_pool_backpressure(pcdn):
         w.e.handle_broadcast_message([0], raw)         # 4 x 3056 > 10 000
     assert ei.value.code == -11                        # PCDN_EAGAIN: the reference would await the semaphore
     assert w.e.stats().inflight_bytes == 3 * len(raw)
+    assert w.e.next_batch() != 0 and w.e.stats().batches == 1   # the refusal launched the open batch (no flush yet)
     got = w.e.drain()                                  # poll + release → permits returned
     assert got[a] == [raw] * 3
     st = w.e.stats()

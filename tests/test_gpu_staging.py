@@ -104,10 +104,12 @@ def test_explicit_batch_refusals(pcdn):
     assert p.e.stats().inflight_bytes == 0 and p.e.stats().bytes_in == 11000
 
 
-def _run_batches(e):
-    """flush, then poll every outstanding batch oldest first: (n_msgs of each batch, {conn: frames})"""
-    e.flush()
-    sizes, out = [], {}
+def _run_batches(e, sizes=None, out=None, flush=True):
+    """flush (unless told not to), then poll every outstanding batch oldest first: (n_msgs of each
+    batch, {conn: frames})"""
+    if flush:
+        e.flush()
+    sizes, out = ([], {}) if sizes is None else (sizes, out)
     while True:
         b = e.next_batch()
         if not b:
@@ -120,16 +122,47 @@ def _run_batches(e):
         e.release_batch(b)
 
 
-@pytest.mark.parametrize("flags", [0, 1], ids=["host-parse", "device-parse"])
-def test_both_receive_paths_cut_the_same_batches(pcdn, flags):
-    """One pcdn_receive_frames call of >= 2048 frames (the threaded path) and the same frames one at a
-    time through user_receive / broker_receive must return the same codes, cut the same batches and
-    deliver the same bytes.  The frames cut batches on the message, byte, broadcast and (host parse)
-    topic-entry limits, with subscribe frames in between.  No memory pool (the two paths react to it
-    differently by design) and enough batch slots that neither path has to drain during the call."""
+def _receive_all(pcdn, e, frames, batched):
+    """Every frame in order: through pcdn_receive_frames calls (`batched`) or one user_receive /
+    broker_receive call each.  Where the engine stops with PCDN_EAGAIN (memory pool exhausted), the
+    batches it launched are drained WITHOUT a flush, and the frames resume where it stopped.  A stop must
+    have launched the batch holding the permits: something is drained, and no message is left in an open
+    batch.  Returns (codes, n_msgs of each batch, {conn: frames}, number of stops)."""
+    n = len(frames)
+    arr = (pcdn.Frame * n)(*[pcdn.Frame(s, len(s), o, raw, len(raw), 0) for s, o, raw in frames])
+    rcs = (C.c_int32 * n)()
+    sizes, out, pos, stops = [], {}, 0, 0
+    while pos < n:
+        if batched:
+            done = e.L.pcdn_receive_frames(e.h, C.cast(C.byref(arr, pos * C.sizeof(pcdn.Frame)), C.POINTER(pcdn.Frame)), n - pos,
+                                           C.cast(C.byref(rcs, pos * 4), C.POINTER(C.c_int32)))
+        else:
+            s, o, raw = frames[pos]
+            rcs[pos] = e.broker_receive("b0/p0", raw) if o else e.user_receive(s, raw)
+            done = EAGAIN if rcs[pos] == EAGAIN else 1
+        assert done == EAGAIN or done > 0
+        pos += max(done, 0)
+        if pos < n and (done == EAGAIN or batched):
+            stops += 1
+            before = len(sizes)
+            _run_batches(e, sizes, out, flush=False)
+            assert len(sizes) > before and e.flush() == 0, "a pool refusal must launch the open batch"
+    _run_batches(e, sizes, out)
+    return list(rcs), sizes, out, stops
+
+
+@pytest.mark.parametrize("flags,pool", [(0, 0), (1, 0), (0, 200_000), (1, 200_000)],
+                         ids=["host-parse", "device-parse", "host-parse-pool", "device-parse-pool"])
+def test_both_receive_paths_cut_the_same_batches(pcdn, flags, pool):
+    """One pcdn_receive_frames call of >= 2048 frames (classified on several threads) and the same frames
+    one at a time through user_receive / broker_receive must return the same codes, cut the same batches
+    and deliver the same bytes.  The frames cut batches on the message, byte, broadcast and (host parse)
+    topic-entry limits, with subscribe frames in between.  Enough batch slots that neither path has to
+    drain during the call; with a global memory pool both stop with PCDN_EAGAIN where it is exhausted,
+    after launching the open batch, and resume once their batches are drained."""
     cfg = dict(max_conns=512, max_topics=256, max_keys=2048, ring_bytes_per_conn=2 << 20, max_batch_msgs=1024,
                max_batch_bcast=300, max_batch_bytes=256 << 10, max_batch_deliveries=1 << 20, batch_slots=48,
-               n_valid_topics=12, flags=flags)
+               n_valid_topics=12, flags=flags, global_memory_pool_size=pool)
     engines = [pcdn.Engine(**cfg), pcdn.Engine(**cfg)]
     try:
         rng = random.Random(17)
@@ -162,14 +195,14 @@ def test_both_receive_paths_cut_the_same_batches(pcdn, flags):
             frames.append((keys[1], j % 2, orc.broadcast_frame([(t + j) % 12 for t in range(3000)], b"t%d" % j)))
         assert len(frames) >= 2048
         a, b = engines
-        rc_a = a.receive_frames([(s, o, raw) for s, o, raw in frames])
-        rc_b = [b.broker_receive("b0/p0", raw) if o else b.user_receive(s, raw) for s, o, raw in frames]
+        rc_a, sizes_a, got_a, stops_a = _receive_all(pcdn, a, frames, batched=True)
+        rc_b, sizes_b, got_b, stops_b = _receive_all(pcdn, b, frames, batched=False)
         assert rc_a == rc_b
-        sizes_a, got_a = _run_batches(a)
-        sizes_b, got_b = _run_batches(b)
         assert sizes_a == sizes_b
         assert got_a == got_b
+        assert stops_a == stops_b and (stops_a >= 3 if pool else stops_a == 0)
         assert 1024 in sizes_a and len(sizes_a) >= 8
+        assert a.stats().bytes_in == b.stats().bytes_in and a.stats().inflight_bytes == b.stats().inflight_bytes == 0
     finally:
         for e in engines:
             e.close()

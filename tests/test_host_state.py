@@ -228,6 +228,57 @@ def test_prune_and_dispatch_errors(pcdn):
     assert e.user_receive(b"u", orc.broadcast_frame([7], b"x")) == -8      # only invalid topics
 
 
+@pytest.mark.parametrize("inbatch", [False, True], ids=["plain", "inbatch-subscribe"])
+def test_receive_frames_call_on_a_host_only_engine(pcdn, inbatch):
+    """One pcdn_receive_frames call of 3000 frames classifies them on several threads, also on a
+    host-only engine.  The frames hold no routable message: Subscribe / Unsubscribe (from users, unknown
+    senders and a peer broker), truncated frames, invalid kinds and topic lists with no valid topic.  The
+    codes, the mirror and pcdn_last_error afterwards equal what the same frames leave one at a time."""
+    flags = pcdn.FLAG_INBATCH_SUBSCRIBE if inbatch else 0
+    rng = random.Random(31)
+    keys = [b"user%03d" % i for i in range(200)]
+    subs = [[rng.randrange(48) for _ in range(rng.randrange(3))] for _ in keys]
+    engines = [pcdn.Engine(device=-1, max_conns=512, max_topics=64, max_keys=1024, n_valid_topics=48, flags=flags)
+               for _ in range(2)]
+    for e in engines:
+        for k, t in zip(keys, subs):
+            e.add_user(k, t)
+        e.add_broker("p/p")
+    frames = []
+    for j in range(3000):
+        sender = rng.choice(keys) if rng.random() < 0.95 else b"stranger%d" % j
+        kind = orc.KIND_SUBSCRIBE if rng.random() < 0.6 else orc.KIND_UNSUBSCRIBE
+        sub = orc.serialize(kind, bytes(rng.randrange(48) for _ in range(rng.randrange(1, 5))))
+        r = rng.random()
+        if r < 0.5:
+            frames.append((sender, 0, sub))
+        elif r < 0.6:                                             # no valid topic: PCDN_EPRUNE
+            frames.append((sender, 0, orc.serialize(kind, bytes(rng.randrange(48, 256) for _ in range(rng.randrange(3))))))
+        elif r < 0.7:                                             # truncated: PCDN_EPARSE
+            frames.append((sender, 0, sub[:rng.randrange(len(sub))]))
+        elif r < 0.8:                                             # PCDN_EKIND
+            frames.append((sender, 0, orc.serialize(rng.choice([orc.KIND_USER_SYNC, orc.KIND_TOPIC_SYNC]), b"", b"x")))
+        else:                                                     # broker origin: not routed here (1)
+            frames.append((b"p/p", 1, sub))
+    frames.append((keys[0], 0, orc.serialize(orc.KIND_USER_SYNC, b"", b"last")))
+    a, b = engines
+    want = [b.broker_receive(s.decode(), raw) if o else b.user_receive(s, raw) for s, o, raw in frames]
+    want_err = pcdn.lib().pcdn_last_error().decode()
+    assert want_err == "invalid message received" and {0, 1, -7, -8, -9} <= set(want)
+    with pytest.raises(pcdn.PcdnError):
+        a.add_user(b"k" * 300, [])                                # leaves another error text behind
+    assert a.receive_frames(frames) == want
+    assert pcdn.lib().pcdn_last_error().decode() == want_err
+
+    def mirror(e):
+        return ([sorted(e.debug_interested([t], to_users_only=uo)) for t in range(64) for uo in (False, True)],
+                sorted(e.get_user_sync(full=True)), sorted(e.get_topic_sync(full=True)), e.num_users())
+
+    assert mirror(a) == mirror(b)
+    for e in engines:
+        e.close()
+
+
 def test_state_calls_from_many_threads(pcdn):
     """the engine serialises callers internally (one mutex = the reference's RwLock<Connections>):
     concurrent add/subscribe/remove from several host threads leave a consistent table"""
