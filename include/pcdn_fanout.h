@@ -401,6 +401,34 @@ int pcdn_handle_broadcast_message(pcdn_engine* e, const uint16_t* topics, uint32
 /* Inner::handle_direct_message handler.rs:197-237 */
 int pcdn_handle_direct_message(pcdn_engine* e, const uint8_t* recipient, uint32_t recipient_len,
                                const uint8_t* raw, uint32_t raw_len, int to_user_only);
+/* ---- data out: the broker's own frames to its peer brokers (cdn-broker/src/tasks/broker/sender.rs) -----
+ * How a host sends the UserSync / TopicSync frames it builds (tasks/broker/sync.rs: the full syncs to a new
+ * peer, the partial syncs to every peer every 10 s) in order with the routed traffic of the same link.
+ *  - Bytes: `raw` is forwarded verbatim, framed as u32 BE len || raw (R1, R2).  The engine does not parse it
+ *    and no message hook runs on it.  It is delivered by the rule of every routed message: a framed copy, or a
+ *    32-byte reference record on PCDN_FLAG_SHARED_PAYLOAD engines and when raw_len >= ref_min_bytes.
+ *  - Place: it is appended to the open batch as ONE message at its position, so every connection's stream
+ *    follows call order together with routed messages (R9).  These are data calls: they do not launch the
+ *    open batch (a full batch is launched and the frame opens the next one, as for any message).
+ *  - Recipients: the peer brokers connected at the call (pcdn_add_broker / pcdn_remove_broker launch the open
+ *    batch first, R12): a broker added after the send does not get the frame; a broker removed after it does
+ *    (its id stays quarantined as usual); after a same-identifier re-add (kick) the frame stays with the old
+ *    connection.  Users never get it; subscriptions, PCDN_FLAG_INBATCH_SUBSCRIBE events and to_users_only
+ *    play no part.  A sharded engine delivers it from each shard to that shard's brokers.
+ *  - Returns 0 = appended; 1 = nothing to send to (no broker `identifier` / no broker connected), nothing
+ *    appended; else the negative codes of pcdn_handle_broadcast_message: PCDN_ENODEV (host-only engine),
+ *    PCDN_EINVAL (length above MAX_MESSAGE_SIZE, or raw NULL with raw_len > 0), PCDN_ENOSPC (does not fit an
+ *    empty batch), PCDN_EAGAIN (no batch slot free).
+ *  - Capacity and counters: one broadcast slot (max_batch_bcast), its arena bytes and its deliveries; counted
+ *    in msgs, deliveries and bytes_out.  It takes NO global_memory_pool_size permits and is not counted in
+ *    bytes_in or inflight_bytes (the reference builds sync frames outside the Limiter, sync.rs:34), so a send
+ *    succeeds while routed frames get PCDN_EAGAIN from the memory pool.  Overflow (overflow_conns), output-pool
+ *    refusal and pcdn_retry_batch work as for any message; a retried batch delivers to the set at launch.
+ *  - pcdn_submit, pcdn_submit_device and pcdn_receive_frames do not carry these messages.                  */
+/* Inner::try_send_to_broker (cdn-broker/src/tasks/broker/sender.rs:17-45) */
+int pcdn_send_to_broker(pcdn_engine* e, const char* identifier, const uint8_t* raw, uint32_t raw_len);
+/* Inner::try_send_to_brokers (sender.rs:49-59): every connected peer broker */
+int pcdn_send_to_brokers(pcdn_engine* e, const uint8_t* raw, uint32_t raw_len);
 /* One iteration of Inner::user_receive_loop (cdn-broker/src/tasks/user/handler.rs:104-161):
  * Message::deserialize (cdn-proto/src/message.rs:212) → Topic::prune (def.rs:36-49) → dispatch.
  * Broadcast/Direct are appended to the open batch; Subscribe/Unsubscribe update the tables (the

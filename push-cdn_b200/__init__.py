@@ -221,6 +221,8 @@ ABI = {
     "pcdn_add_users_bulk": (_ci, [_vp, _vp, _u32, _u32, _u32, _vp, _vp, _vp]),
     "pcdn_handle_broadcast_message": (_ci, [_vp, _u16p, _u32, _u8p, _u32, _ci]),
     "pcdn_handle_direct_message": (_ci, [_vp, _u8p, _u32, _u8p, _u32, _ci]),
+    "pcdn_send_to_broker": (_ci, [_vp, _cp, _u8p, _u32]),
+    "pcdn_send_to_brokers": (_ci, [_vp, _u8p, _u32]),
     "pcdn_user_receive": (_ci, [_vp, _u8p, _u32, _u8p, _u32]),
     "pcdn_broker_receive": (_ci, [_vp, _cp, _u8p, _u32]),
     "pcdn_set_message_hook": (_ci, [_vp, _ci, MESSAGE_HOOK, _vp]),
@@ -460,6 +462,16 @@ class Engine:
 
     def handle_direct_message(self, recipient: bytes, raw: bytes, to_user_only: bool = False) -> None:
         self._chk(self.L.pcdn_handle_direct_message(self.h, recipient, len(recipient), raw, len(raw), int(to_user_only)))
+
+    # ---- data out: the broker's own frames to its peer brokers (tasks/broker/sender.rs) --------
+    def send_to_broker(self, ident: str, raw: bytes) -> int:
+        """Inner::try_send_to_broker: `raw` (e.g. a UserSync or TopicSync frame, forwarded verbatim) to the
+        peer broker `ident`, in order with the open batch's routed messages.  0 = appended, 1 = no such broker."""
+        return self._chk(self.L.pcdn_send_to_broker(self.h, ident.encode(), raw, len(raw)))
+
+    def send_to_brokers(self, raw: bytes) -> int:
+        """Inner::try_send_to_brokers: `raw` to every connected peer broker.  0 = appended, 1 = no broker."""
+        return self._chk(self.L.pcdn_send_to_brokers(self.h, raw, len(raw)))
 
     def set_message_hook(self, origin: int, fn) -> None:
         """MessageHookDef (cdn-proto/src/def.rs:79-92).  fn(msg: HookMessage) -> HOOK_PROCESS | HOOK_SKIP | negative

@@ -106,7 +106,7 @@ int flush_journal(pcdn_engine* e) {
 }
 
 void slot_reset_open(Slot& s) {
-  s.arena_used = 0; s.n_direct = 0; s.devparse = false; s.ingress_bytes = 0; s.n_msgs = 0; s.max_raw_len = 0;
+  s.arena_used = 0; s.n_direct = 0; s.devparse = false; s.ingress_bytes = 0; s.n_msgs = 0; s.max_raw_len = 0; s.targeted = false;
   s.kind.clear(); s.flags.clear(); s.slot_off16.clear(); s.raw_len.clear(); s.aux_off.clear(); s.aux_len.clear();
   s.bcast_index.clear(); s.topics.clear(); s.events.clear(); s.ev_topics.clear();
   s.device_input = false; s.counted = false;
@@ -201,6 +201,7 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   sh.prev_slot[0] = (int)si;
   cudaStream_t st = sh.stream, ps = (!dp && (direct_only || fat_overlap)) ? sh.pack_stream : sh.stream, cs = sh.copy_stream;
   const bool has_direct = n_direct > 0;
+  const Slot& hs = e->slots[si];
   if (wait_ingest) CUDA_TRY(cudaStreamWaitEvent(st, s.ev_ingest, 0));
   s.timed = e->timing;
   s.polled = false;
@@ -242,10 +243,10 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   }
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[1], st));
   if (fused) {
-    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, zero_in_kernel, s.d_stats_pub, retry, st);
+    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, hs.targeted, zero_in_kernel, s.d_stats_pub, retry, st);
     if (s.timed) { CUDA_TRY(cudaEventRecord(s.ev[2], st)); CUDA_TRY(cudaEventRecord(s.ev[3], st)); }
   } else {
-    if (!retry) launch_match(sh.dev, s.w, s.in, zero_in_match ? s.w.stats : nullptr, st);
+    if (!retry) launch_match(sh.dev, s.w, s.in, zero_in_match ? s.w.stats : nullptr, hs.targeted, st);
     if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[2], st));
     if (!retry) launch_plan(sh.dev, s.w, s.in, st);
     launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);   // pool mode: a pure function of the scratch
@@ -272,7 +273,6 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   // batch without a pack launch copies them
   // engines with ref_min_bytes: a host-staged batch runs k_pack_ref only when a message reaches the threshold; the
   // lengths of a device-resident batch are on the device, so it always does
-  const Slot& hs = e->slots[si];
   const bool has_ref = e->cfg.ref_min_bytes && (hs.device_input || hs.max_raw_len >= e->cfg.ref_min_bytes);
   const bool published = launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, has_ref, fused ? nullptr : s.d_stats_pub, ps);
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[5], ps));
@@ -440,15 +440,17 @@ struct BatchFill {
   uint64_t bytes = 0, topics = 0, ingress = 0;
   uint64_t ev_topics = 0;   // topic entries of the batch's subscription events (they share the topic capacity)
   uint32_t max_raw_len = 0;
+  bool targeted = false;    // some message carries MSGF_TARGET
   void add(const MsgShape& m) {
     msgs++; bcast += m.kind == PCDN_KIND_BROADCAST ? 1 : 0;
-    bytes += m.bytes(); topics += m.n_topics; ingress += m.raw_len;
+    bytes += m.bytes(); topics += m.n_topics; ingress += m.ingress();
     max_raw_len = std::max(max_raw_len, m.raw_len);
+    targeted |= m.target;
   }
 };
 BatchFill fill_of(const Slot& s) {
   return BatchFill{(uint32_t)s.kind.size(), (uint32_t)s.bcast_index.size(), s.arena_used, s.topics.size(), 0, s.ev_topics.size(),
-                   s.max_raw_len};
+                   s.max_raw_len, s.targeted};
 }
 
 // The per-batch limits: nullptr when `m` still fits a batch that holds `f`, else the limit it would
@@ -514,9 +516,9 @@ int sub_change(pcdn_engine* e, SubOp op, const std::string& who, const uint16_t*
 }
 
 // a frame this engine never accepts (PCDN_EINVAL): the reason, else nullptr
-const char* msg_invalid(const pcdn_engine* e, uint32_t raw_len) {
-  if (raw_len > 0x1FFFFFFFu) return "message larger than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25)";
-  if (e->cfg.global_memory_pool_size && raw_len > e->cfg.global_memory_pool_size) return "message larger than the global memory pool";
+const char* msg_invalid(const pcdn_engine* e, const MsgShape& m) {
+  if (m.raw_len > 0x1FFFFFFFu) return "message larger than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25)";
+  if (e->cfg.global_memory_pool_size && m.ingress() > e->cfg.global_memory_pool_size) return "message larger than the global memory pool";
   return nullptr;
 }
 
@@ -538,7 +540,7 @@ void as_batch(Entry& p, InMsg& m) {
   if (m.kind == PCDN_KIND_DIRECT)
     m.stage_key |= !(m.key && m.key >= m.raw && m.key + m.key_len <= m.raw + m.raw_len && ((m.key - m.raw) & 3) == 0);
   p.route = ROUTE_BATCH; p.devparse = (m.flags & MSGF_DEVPARSE) != 0; p.rc = 0; p.why = nullptr;
-  p.shape = MsgShape{m.kind, m.raw_len, m.stage_key ? (uint32_t)align_up(m.key_len, 16) : 0u, m.n_topics};
+  p.shape = MsgShape{m.kind, m.raw_len, m.stage_key ? (uint32_t)align_up(m.key_len, 16) : 0u, m.n_topics, (m.flags & MSGF_TARGET) != 0};
 }
 
 // Scratch entry i as a message of the C ABI's handle / submit calls.  A multi-process group stages every
@@ -658,7 +660,7 @@ void write_msg(Slot& s, const Entry& p, const InMsg& m, uint32_t n_valid) {
     s.aux_len[mi] = m.key_len;
     return;
   }
-  s.aux_off[mi] = p.topic_off;
+  s.aux_off[mi] = (m.flags & MSGF_TARGET) ? m.target : p.topic_off;
   s.aux_len[mi] = m.n_topics;
   s.bcast_index[p.bcast_pos] = mi;
   for (uint32_t t = 0, k = p.topic_off; t < m.n_listed; t++) {
@@ -670,6 +672,7 @@ void write_msg(Slot& s, const Entry& p, const InMsg& m, uint32_t n_valid) {
 // the open slot `s` now holds `f`: messages up to f.msgs are written
 void slot_commit(pcdn_engine* e, Slot& s, const BatchFill& f, bool devparse) {
   s.arena_used = f.bytes; s.n_direct = f.msgs - f.bcast; s.devparse |= devparse; s.max_raw_len = f.max_raw_len;
+  s.targeted = f.targeted;
   s.ingress_bytes += f.ingress; e->inflight_bytes += f.ingress; e->stats.bytes_in += f.ingress;
 }
 
@@ -727,7 +730,7 @@ int place_entries(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t*
     if (p.route == ROUTE_BATCH) {
       const char* why;
       if (!e->has_device) rc = fail(PCDN_ENODEV, "host-only engine cannot route messages");
-      else if ((why = msg_invalid(e, p.shape.raw_len))) rc = fail(PCDN_EINVAL, why);
+      else if ((why = msg_invalid(e, p.shape))) rc = fail(PCDN_EINVAL, why);
       else if ((why = batch_limit(e, BatchFill{}, p.shape))) rc = fail(PCDN_ENOSPC, std::string("message does not fit an empty batch: ") + why);
       else for (bool launched = false;; launched = true) {   // the open batch, else a new one behind it
         if (!open) {
@@ -735,7 +738,7 @@ int place_entries(pcdn_engine* e, const pcdn_frame* frames, uint32_t n, int32_t*
           fill = fill_of(e->slots[e->open_slot]);
           open = true; run = i;
         }
-        if (!batch_limit(e, fill, p.shape) && pool_admits(e, fill.ingress + p.shape.raw_len)) {
+        if (!batch_limit(e, fill, p.shape) && pool_admits(e, fill.ingress + p.shape.ingress())) {
           p.msg_idx = fill.msgs; p.arena_off = fill.bytes; p.bcast_pos = fill.bcast; p.topic_off = (uint32_t)fill.topics;
           fill.add(p.shape);
           devparse |= p.devparse;
@@ -1372,6 +1375,44 @@ int pcdn_handle_direct_message(pcdn_engine* e, const uint8_t* recipient, uint32_
   GUARD_END
 }
 
+// ---- data out: frames the broker itself sends to its peer brokers ------------------------------
+namespace {
+// Inner::try_send_to_broker / try_send_to_brokers (tasks/broker/sender.rs:17-59): `raw` as one broadcast slot of
+// the open batch whose recipients are the broker `identifier` (null: every peer broker) as connected now.  The
+// mirror names the recipients: add_broker / remove_broker launch the open batch first (R12), so the batch is
+// routed against this same set.  1 = nothing to send to (no such broker / no broker at all): nothing is appended.
+int send_to_brokers(pcdn_engine* e, const char* identifier, const uint8_t* raw, uint32_t raw_len) {
+  if (raw_len && !raw) return fail(PCDN_EINVAL, "null frame with non-zero length");
+  if (const char* why = msg_invalid(e, MsgShape{PCDN_KIND_BROADCAST, raw_len, 0, 0, true})) return fail(PCDN_EINVAL, why);
+  if (!e->has_device) return fail(PCDN_ENODEV, "host-only engine cannot route messages");
+  uint32_t target = kConnNone;
+  if (identifier) {
+    target = e->conns->broker_conn(identifier);
+    if (target == PCDN_CONN_NONE) return 1;   // if let Some(connection) = connection (sender.rs:29)
+  } else if (e->conns->num_brokers() == 0) {
+    return 1;                                 // the loop over no broker (sender.rs:52-57)
+  }
+  e->rx_reserve(1);
+  api_entry(e, 0, PCDN_KIND_BROADCAST, MSGF_TARGET, nullptr, 0, nullptr, 0, raw, raw_len);
+  e->rx_msgs[0].target = target;
+  place_entries(e, nullptr, 1, nullptr, false);
+  return e->rx_plan[0].rc;
+}
+}  // namespace
+
+int pcdn_send_to_broker(pcdn_engine* e, const char* identifier, const uint8_t* raw, uint32_t raw_len) {
+  GUARD_BEGIN
+  LOCK;
+  return send_to_brokers(e, identifier ? identifier : "", raw, raw_len);   // (BrokerIdent::parse reads null as "")
+  GUARD_END
+}
+int pcdn_send_to_brokers(pcdn_engine* e, const uint8_t* raw, uint32_t raw_len) {
+  GUARD_BEGIN
+  LOCK;
+  return send_to_brokers(e, nullptr, raw, raw_len);
+  GUARD_END
+}
+
 int pcdn_user_receive(pcdn_engine* e, const uint8_t* sender_key, uint32_t key_len, const uint8_t* raw, uint32_t raw_len) {
   GUARD_BEGIN
   LOCK;
@@ -1430,10 +1471,10 @@ static int validate_explicit_batch(pcdn_engine* e, const pcdn_msg* msgs, uint32_
     if ((m.raw_len && !m.raw) || (m.kind == PCDN_KIND_BROADCAST && m.n_topics && !m.topics) ||
         (m.kind == PCDN_KIND_DIRECT && m.recipient_len && !m.recipient))
       return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": null pointer with non-zero length");
-    if (const char* why = msg_invalid(e, m.raw_len)) return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": " + why);
     const bool direct = m.kind == PCDN_KIND_DIRECT;
     const MsgShape shape{m.kind, m.raw_len, direct ? (uint32_t)align_up(std::min<uint32_t>(m.recipient_len, c.max_key_len + 1), 16) : 0u,
                          direct ? 0u : m.n_topics};
+    if (const char* why = msg_invalid(e, shape)) return fail(PCDN_EINVAL, "message " + std::to_string(i) + ": " + why);
     if (!full) full = batch_limit(e, fill, shape);
     fill.add(shape);
   }

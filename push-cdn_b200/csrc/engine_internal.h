@@ -146,6 +146,7 @@ struct Slot {
   std::chrono::steady_clock::time_point t_launch;
   bool devparse = false;        // some messages carry MSGF_DEVPARSE (k_parse runs first)
   uint32_t max_raw_len = 0;     // host-staged: longest message (with ref_min_bytes: whether k_pack_ref runs)
+  bool targeted = false;        // host-staged: some message carries MSGF_TARGET (pcdn_send_to_broker(s))
   bool counted = false;         // counters of this batch have been added to the engine stats
   // merged view of a sharded batch for pcdn_poll (host copy of the shards' span tables)
   std::vector<pcdn_span> merged_spans;
@@ -159,6 +160,7 @@ struct InMsg {
   bool prune;                        // broadcast: apply Topic::prune to the wire topic list
   bool stage_key;                    // direct: the recipient is copied beside the frame, not read in place
   uint32_t raw_len, key_len;         // key_len: direct message's recipient length (routed_key_len)
+  uint32_t target;                   // MSGF_TARGET: the recipient connection (global id), kConnNone = every peer broker
   uint32_t n_listed, n_topics;       // broadcast: entries of the topic list below, entries it adds to the batch
   const uint8_t* raw;
   const uint8_t* key;                // direct: the recipient
@@ -168,9 +170,13 @@ struct InMsg {
 
 // What one message adds to a batch: a 16-byte frame slot (4-byte length hole, raw bytes, zero pad),
 // `key_bytes` of recipient key staged beside it (0 when the key is read in place) and topic entries.
+// `target`: a MSGF_TARGET message, which takes no memory-pool permits (the reference builds sync frames
+// outside the Limiter, tasks/broker/sync.rs:34).
 struct MsgShape {
   uint8_t kind;
   uint32_t raw_len, key_bytes, n_topics;
+  bool target;
+  uint64_t ingress() const { return target ? 0 : raw_len; }
   size_t bytes() const { return align_up(4 + (size_t)raw_len, 16) + key_bytes; }
 };
 

@@ -432,10 +432,23 @@ __device__ __forceinline__ void apply_events(const DevState& s, const BatchIn& b
   }
 }
 
+// match word `wd` of a MSGF_TARGET message m (pcdn_send_to_broker(s)): the shard's broker mask for "every peer
+// broker", else the bit of its one target connection (0 when that connection lies outside this shard's slice).
+// No topic rows, in-batch events or to_users_only: the recipients are the brokers connected when it was sent.
+__device__ __forceinline__ uint32_t target_word(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd) {
+  const uint32_t c = b.aux_off[m];
+  if (c == kConnNone) return s.brk[wd];
+  const uint32_t local = c - s.conn_base;   // (unsigned wrap: below the base → outside the slice)
+  return local < s.N && (local >> 5) == wd ? 1u << (local & 31u) : 0u;
+}
+
 // match word `wd` (32 connections) of message m: OR of its topics' bitmap rows (a2)
+// (TARGET: the batch holds a MSGF_TARGET message; only that instantiation reads the flag)
+template <bool TARGET>
 __device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd) {
   const uint32_t toff = b.aux_off[m], tn = b.aux_len[m];
   const uint32_t fl = b.flags[m];
+  if (TARGET && (fl & MSGF_TARGET)) return target_word(s, b, m, wd);
   uint32_t word = 0;
   if (fl & MSGF_TOPICS_U8) {  // wire topic list read in place (device-parse mode)
     const uint8_t* tb = b.arena + toff;
@@ -457,7 +470,7 @@ __device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn&
 // Warp = one 256-word match block of one message, lane = 8 consecutive words (32-byte vector
 // loads of the bitmap rows, no block-level synchronisation: the popcount prefix of a 256-word block
 // is a lane-local prefix plus one warp scan).  grid = (ceil(nblk / 8), n_bcast).
-template <bool EVENTS>
+template <bool EVENTS, bool TARGET>
 __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, BatchStats* zero) {
   // the batch's first kernel when it has no direct message and no device parse: it zeroes the counters
   // (nothing else in this launch touches them) instead of a memset on the stream
@@ -485,7 +498,7 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, Ba
   } else {
     for (uint32_t i = 0; i < tn; i++) or_row(b.topics[toff + i]);
   }
-  if (EVENTS) {
+  if (EVENTS && !(TARGET && (fl & MSGF_TARGET))) {
     uint32_t v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
     apply_events<8>(s, b, m, w0, v);
     lo = make_uint4(v[0], v[1], v[2], v[3]); hi = make_uint4(v[4], v[5], v[6], v[7]);
@@ -495,6 +508,19 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, Ba
     const uint4 a = br[0], c = br[1];
     lo.x &= ~a.x; lo.y &= ~a.y; lo.z &= ~a.z; lo.w &= ~a.w;
     hi.x &= ~c.x; hi.y &= ~c.y; hi.z &= ~c.z; hi.w &= ~c.w;
+  }
+  // pcdn_send_to_broker(s): the target's row (target_word, eight words at once).  A MSGF_TARGET message lists no
+  // topic and is never to_users_only, so lo / hi are still zero here.
+  if (TARGET && (fl & MSGF_TARGET)) {
+    if (toff == kConnNone) {
+      const uint4* br = reinterpret_cast<const uint4*>(s.brk + w0);
+      lo = br[0]; hi = br[1];
+    } else {
+      const uint32_t local = toff - s.conn_base, bit = 1u << (local & 31u);
+      const uint32_t q = local < s.N ? (local >> 5) - w0 : 8u;   // (unsigned: a word before w0 is >= 8 too)
+      lo = make_uint4(q == 0 ? bit : 0u, q == 1 ? bit : 0u, q == 2 ? bit : 0u, q == 3 ? bit : 0u);
+      hi = make_uint4(q == 4 ? bit : 0u, q == 5 ? bit : 0u, q == 6 ? bit : 0u, q == 7 ? bit : 0u);
+    }
   }
   const uint32_t p0 = __popc(lo.x), p1 = p0 + __popc(lo.y), p2 = p1 + __popc(lo.z), p3 = p2 + __popc(lo.w);
   const uint32_t p4 = p3 + __popc(hi.x), p5 = p4 + __popc(hi.y), p6 = p5 + __popc(hi.z), p7 = p6 + __popc(hi.w);
@@ -527,13 +553,18 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, Ba
     if (lane == 0) { w.D[m] = carry; w.jidx[m] = j; w.done[j] = 0; }
   }
 }
-void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, cudaStream_t st) {
+void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, bool targeted, cudaStream_t st) {
   if (!b.n_bcast) return;
   dim3 grid((s.nblk + 7) / 8, b.n_bcast);
-  // (a batch with in-batch subscription events takes its own instantiation: the one without them keeps
-  //  the registers and occupancy it has without the patch)
-  if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true><<<grid, 256, 0, st>>>(s, b, w, zero);
-  else PCDN_COUNT_LAUNCH, k_match<false><<<grid, 256, 0, st>>>(s, b, w, zero);
+  // (a batch with in-batch subscription events, or with a targeted message, takes its own instantiation: the
+  //  one without them keeps the registers and occupancy it has without the patch or the target rows)
+  if (targeted) {
+    if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true, true><<<grid, 256, 0, st>>>(s, b, w, zero);
+    else PCDN_COUNT_LAUNCH, k_match<false, true><<<grid, 256, 0, st>>>(s, b, w, zero);
+  } else {
+    if (b.n_events) PCDN_COUNT_LAUNCH, k_match<true, false><<<grid, 256, 0, st>>>(s, b, w, zero);
+    else PCDN_COUNT_LAUNCH, k_match<false, false><<<grid, 256, 0, st>>>(s, b, w, zero);
+  }
 }
 
 // =============================================================================== K1p plan
@@ -1018,7 +1049,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 }
 // offsets_only: the retry of a batch the output pool refused — the routing of the first run (direct
 // bounds, match words, plan) is still in the scratch, only the offsets pass runs again.
-template <bool HAS_DIRECT>
+template <bool HAS_DIRECT, bool TARGET>
 __global__ void __cluster_dims__(8, 1, 1) __launch_bounds__(1024, 1)
 k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish, int offsets_only) {
   __shared__ uint32_t sm[33];
@@ -1059,7 +1090,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish,
       const bool live = it < nitems;
       const uint32_t j = live ? it / s.nblk : 0, blk = live ? it % s.nblk : 0;
       const uint32_t wd = blk * kBlockWords + wl;
-      const uint32_t word = live ? match_word(s, b, b.bcast_index[j], wd) : 0;
+      const uint32_t word = live ? match_word<TARGET>(s, b, b.bcast_index[j], wd) : 0;
       uint32_t tot, ex = cta_excl_scan<32>(__popc(word), &tot, sm);
       if (wl == 0) gbase[q] = ex;
       if (tid == 0) gbase[4] = tot;
@@ -1129,10 +1160,16 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish,
       reinterpret_cast<uint32_t*>(publish)[tid] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + tid);
   }
 }
-void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool zero_stats,
+void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, bool zero_stats,
                        BatchStats* publish, bool offsets_only, cudaStream_t st) {
-  if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish, offsets_only ? 1 : 0);
-  else PCDN_COUNT_LAUNCH, k_ctrl_small<false><<<8, 1024, 0, st>>>(s, b, w, zero_stats ? 1 : 0, publish, offsets_only ? 1 : 0);
+  const int z = zero_stats ? 1 : 0, oo = offsets_only ? 1 : 0;
+  if (targeted) {   // (as in launch_match: the instantiations without target rows stay as they are)
+    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, true><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, true><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+  } else {
+    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, false><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, false><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+  }
 }
 
 // Pool mode, retry of a refused batch: the offsets pass runs again from the counters as the plan left

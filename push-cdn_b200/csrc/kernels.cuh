@@ -8,7 +8,8 @@
 //                       connection's segment (no sort: the connection's thread orders its few entries
 //                       in k_offsets; k_dsort_hot orders connections with > 32 hits by bitmap)
 //   K1a k_match         OR of subscription-bitmap rows per broadcast → match words + popcount ranks
-//                       (bits of connections with in-batch subscription events re-evaluated per message)
+//                       (bits of connections with in-batch subscription events re-evaluated per message;
+//                       a MSGF_TARGET message's row is the broker mask or its one target connection's bit)
 //   K1p k_plan_*        D_m per message, class (thin / message-major / connection-major), scatter-list
 //                       bases and pack tiles by prefix sums (one launch when <= 256 messages)
 //   K1b k_offsets       thread per connection walks the batch IN ORDER (R9), assigns ring offsets and
@@ -63,7 +64,11 @@ enum : uint8_t {
   MSGF_USERS_ONLY = 1,
   MSGF_DEVPARSE = 2,   // k_parse fills kind / aux_off / aux_len from the raw frame
   MSGF_TOPICS_U8 = 4,  // aux_off = byte offset in the arena of the wire topic list (u8 each)
-  MSGF_PRUNE = 8       // user-origin: apply Topic::prune while reading the wire topic list
+  MSGF_PRUNE = 8,      // user-origin: apply Topic::prune while reading the wire topic list
+  // pcdn_send_to_broker(s): a broadcast slot whose match row is its target, not topic rows: aux_off = the target's
+  // global connection id, or kConnNone for every peer broker of the shard; aux_len = 0.  Read only by the
+  // instantiations a batch holding such a message selects (launch_match / launch_ctrl_small: `targeted`)
+  MSGF_TARGET = 16
 };
 constexpr int8_t kErrParse = -7, kErrPrune = -8;  // PCDN_EPARSE / PCDN_EPRUNE
 
@@ -243,11 +248,12 @@ void launch_batch_begin(const DevState& s, const Work& w, const BatchIn& b, bool
 void launch_parse(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st);
 // zero: the batch's counters, zeroed by k_match before any kernel writes one (null: zeroed earlier)
-void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, cudaStream_t st);
+// targeted: the batch holds a MSGF_TARGET message (host-staged batches only)
+void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, bool targeted, cudaStream_t st);
 void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st);
 // fused match + plan + offsets for N <= kSmallCtrlConns and n_msgs <= kSmallCtrlMsgs (one cluster launch)
-void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool zero_stats,
+void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, bool zero_stats,
                        BatchStats* publish, bool offsets_only, cudaStream_t st);
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);

@@ -1,0 +1,116 @@
+"""pcdn_send_to_broker / pcdn_send_to_brokers without a GPU: the restatement of Inner::try_send_to_broker /
+try_send_to_brokers (cdn-broker/src/tasks/broker/sender.rs:17-59) on the oracle that the GPU tests compare
+against, the host-only engine's answer and the argument checks that come before it."""
+import ctypes as C
+
+import pytest
+
+from oracle import oracle as orc
+
+ENODEV, EINVAL = -3, -1
+
+
+def relay_key(ident):
+    """a DirectMap key owned by peer broker `ident` (no user key of these tests starts with 0xFF 0x00)"""
+    return b"\xff\x00send-to:" + ident.encode()
+
+
+def try_send_to_broker(o, ident, raw):
+    """Inner::try_send_to_broker (sender.rs:17-45) on oracle `o`; 1 = no such broker (nothing sent).
+    The frame goes through the oracle's own send path: handle_direct_message (tasks/broker/handler.rs:197-237)
+    of a key that `ident` owns ends in try_send_to_broker(ident) → send_message_raw on that broker's connection,
+    so the frame takes its place in the broker's stream in call order with everything routed to it."""
+    if o.broker_conn(ident) < 0:
+        return 1                                       # if let Some(connection) = connection (sender.rs:29)
+    key = relay_key(ident)
+    o.apply_user_sync(ident, [(key, 1, ident)])        # (no local user has the key: nobody is removed)
+    o.handle_direct_message(key, raw)
+    return 0
+
+
+def try_send_to_brokers(o, idents, raw):
+    """Inner::try_send_to_brokers (sender.rs:49-59): try_send_to_broker for every connected broker.  `idents`: the
+    identifiers ever added (the oracle does not list its brokers); 1 = none of them is connected."""
+    live = [i for i in dict.fromkeys(idents) if o.broker_conn(i) >= 0]
+    for i in live:
+        try_send_to_broker(o, i, raw)
+    return 0 if live else 1
+
+
+def framed(raw):
+    return len(raw).to_bytes(4, "big") + raw
+
+
+@pytest.fixture
+def sync_frames():
+    """a UserSync and a TopicSync message as the host builds them (the engine never parses them)"""
+    return (orc.serialize(orc.KIND_USER_SYNC, b"", b"user-sync archive" * 7),
+            orc.serialize(orc.KIND_TOPIC_SYNC, b"", b"topic-sync archive" * 3))
+
+
+def test_oracle_sends_to_one_broker_and_to_every_broker(sync_frames):
+    us, ts = sync_frames
+    o = orc.Oracle("/")
+    user = o.add_user(b"u" * 32, [0, 1])
+    a, b, c = o.add_broker("a/a"), o.add_broker("b/b"), o.add_broker("c/c")
+    o.subscribe_broker_to("a/a", [0])          # subscriptions play no part
+    assert try_send_to_broker(o, "b/b", ts) == 0
+    assert try_send_to_brokers(o, ["a/a", "b/b", "c/c"], us) == 0
+    assert o.stream(a) == framed(us)
+    assert o.stream(b) == framed(ts) + framed(us)
+    assert o.stream(c) == framed(us)
+    assert o.stream(user) == b""               # users never get these frames
+    assert o.deliveries() == 4 and o.bytes_sent() == len(ts) + 3 * len(us)
+
+
+def test_oracle_unknown_identifier_and_no_broker(sync_frames):
+    us, _ = sync_frames
+    o = orc.Oracle("/")
+    user = o.add_user(b"u" * 32, [0])
+    assert try_send_to_brokers(o, [], us) == 1          # the loop over no broker (sender.rs:52-57)
+    a = o.add_broker("a/a")
+    assert try_send_to_broker(o, "x/x", us) == 1        # if let Some(connection) (sender.rs:29)
+    assert try_send_to_brokers(o, ["x/x"], us) == 1
+    assert o.stream(a) == b"" and o.stream(user) == b"" and o.deliveries() == 0
+
+
+def test_oracle_removed_broker_and_kick(sync_frames):
+    us, ts = sync_frames
+    o = orc.Oracle("/")
+    a, b = o.add_broker("a/a"), o.add_broker("b/b")
+    o.remove_broker("a/a")
+    assert try_send_to_broker(o, "a/a", us) == 1
+    assert try_send_to_brokers(o, ["a/a", "b/b"], ts) == 0
+    assert o.stream(a) == b"" and o.stream(b) == framed(ts)
+    b2 = o.add_broker("b/b")                   # same identifier again: the old connection is kicked
+    assert b2 != b and o.conn_removed(b)
+    assert try_send_to_broker(o, "b/b", us) == 0
+    assert o.stream(b) == framed(ts) and o.stream(b2) == framed(us)
+    assert o.num_users() == 0                           # the relay keys are no users
+
+
+def test_host_only_engine_refuses_with_enodev(pcdn, sync_frames):
+    us, _ = sync_frames
+    e = pcdn.Engine(device=-1)
+    e.add_broker("a/a")
+    for call in (lambda: e.send_to_broker("a/a", us), lambda: e.send_to_brokers(us)):
+        with pytest.raises(pcdn.PcdnError) as ei:
+            call()
+        assert ei.value.code == ENODEV
+        assert "host-only" in e.L.pcdn_last_error().decode()
+    e.close()
+
+
+def test_bad_arguments(pcdn):
+    e = pcdn.Engine(device=-1)
+    e.add_broker("a/a")
+    L = e.L
+    assert L.pcdn_send_to_brokers(e.h, None, 5) == EINVAL
+    assert "null frame" in L.pcdn_last_error().decode()
+    assert L.pcdn_send_to_broker(e.h, b"a/a", None, 1) == EINVAL
+    buf = C.create_string_buffer(16)
+    # longer than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25): refused before the frame is read
+    assert L.pcdn_send_to_brokers(e.h, C.cast(buf, C.c_char_p), 0x20000000) == EINVAL
+    assert "MAX_MESSAGE_SIZE" in L.pcdn_last_error().decode()
+    assert L.pcdn_send_to_broker(e.h, None, C.cast(buf, C.c_char_p), 0x20000000) == EINVAL
+    e.close()
