@@ -696,7 +696,9 @@ struct ConnCursor {
 __device__ __forceinline__ uint32_t alloc_record(ConnCursor& k, uint32_t u, uint32_t R, uint32_t raw_len) {
   if (k.ovf) return kOffInvalid;
   const bool wrap = k.pt + u > R;
-  const uint32_t pad = wrap ? R - k.pt : 0, at = wrap ? 0 : k.pt;
+  // a drained ring (nothing in use) wraps for free: the space before its tail is free as well, so any
+  // record of at most R units fits it (us == 0 also means no record of this batch is placed yet)
+  const uint32_t pad = (wrap && k.us) ? R - k.pt : 0, at = wrap ? 0 : k.pt;
   if (u > R || k.us + pad + u > R) { k.ovf = 1; return kOffInvalid; }
   k.us += pad + u;
   k.bu += pad + u;
