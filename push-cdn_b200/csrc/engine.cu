@@ -237,13 +237,13 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
   if (retry) {
     launch_pool_retry_begin(sh.dev, s.w, st);
   } else {
-    if (!zero_in_kernel && !zero_in_match) launch_batch_begin(sh.dev, s.w, s.in, has_direct, st);
+    if (!zero_in_kernel && !zero_in_match) launch_batch_begin(s.w, st);
     if (devparse) launch_parse(sh.dev, s.w, s.in, st);
     if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
   }
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[1], st));
   if (fused) {
-    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, hs.targeted, zero_in_kernel, s.d_stats_pub, retry, st);
+    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, hs.targeted, zero_in_kernel ? s.w.stats : nullptr, s.d_stats_pub, retry, st);
     if (s.timed) { CUDA_TRY(cudaEventRecord(s.ev[2], st)); CUDA_TRY(cudaEventRecord(s.ev[3], st)); }
   } else {
     if (!retry) launch_match(sh.dev, s.w, s.in, zero_in_match ? s.w.stats : nullptr, hs.targeted, st);

@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(256) k_dsort_hot(BatchIn b, Work w, uint32_t w
   }
 }
 
-void launch_batch_begin(const DevState&, const Work& w, const BatchIn&, bool, cudaStream_t st) {
+void launch_batch_begin(const Work& w, cudaStream_t st) {
   cudaMemsetAsync(w.stats, 0, sizeof(BatchStats), st);
 }
 
@@ -373,36 +373,43 @@ void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t 
 // ---- in-batch subscription events (PCDN_FLAG_INBATCH_SUBSCRIBE).  The bitmap holds every connection's
 // membership as it was when the batch was opened; a connection with events gets its bit of message m
 // re-evaluated: per topic of m, its membership before the batch with its events at positions <= m
-// replayed in order, ORed over the topics.  Both match paths patch their words before the popcounts, so
-// ranks, plan, offsets and pack see the patched bits like any other.
+// replayed in order, ORed over the topics.  The match patches its words before the popcounts, so ranks,
+// plan, offsets and pack see the patched bits like any other.
 
-// topic i of message m's list (toff, fl: m's aux_off, flags): false when Topic::prune drops it or it names no row
-__device__ __forceinline__ bool msg_topic(const DevState& s, const BatchIn& b, uint32_t fl, uint32_t toff, uint32_t i, uint32_t* t) {
+// every bitmap row message m names (fl, toff, tn: m's flags, aux_off, aux_len), in list order: the wire u8 list
+// read in place with Topic::prune applied (device-parse mode), or the host's u16 list; a topic naming no row is
+// skipped.  f(t) returns true to stop the walk.
+template <class F>
+__device__ __forceinline__ void for_each_topic(const DevState& s, const BatchIn& b, uint32_t fl, uint32_t toff, uint32_t tn, F&& f) {
   if (fl & MSGF_TOPICS_U8) {
     const uint8_t* tb = b.arena + toff;
-    if ((fl & MSGF_PRUNE) && !topic_kept(tb, i, s.n_valid_topics)) return false;
-    *t = tb[i];
+    for (uint32_t i = 0; i < tn; i++) {
+      if ((fl & MSGF_PRUNE) && !topic_kept(tb, i, s.n_valid_topics)) continue;
+      const uint32_t t = tb[i];
+      if (t < s.T && f(t)) return;
+    }
   } else {
-    *t = b.topics[toff + i];
+    for (uint32_t i = 0; i < tn; i++) {
+      const uint32_t t = b.topics[toff + i];
+      if (t < s.T && f(t)) return;
+    }
   }
-  return *t < s.T;
 }
 
 // bit k of local word wd for message m, with the connection's events [e0, e1) (its events at positions <= m)
 __device__ uint32_t event_bit(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd, uint32_t k, uint32_t e0, uint32_t e1) {
-  const uint32_t fl = b.flags[m], toff = b.aux_off[m], tn = b.aux_len[m];
-  for (uint32_t i = 0; i < tn; i++) {
-    uint32_t t;
-    if (!msg_topic(s, b, fl, toff, i, &t)) continue;
+  uint32_t bit = 0;
+  for_each_topic(s, b, b.flags[m], b.aux_off[m], b.aux_len[m], [&](uint32_t t) {
     uint32_t on = (s.sub[(size_t)t * s.W + wd] >> k) & 1u;
     for (uint32_t e = e0; e < e1; e++) {
       const SubEvent ev = b.events[e];
       for (uint32_t q = 0; q < ev.tn; q++)
         if (b.ev_topics[ev.toff + q] == t) { on = ev.pos_op >> 31; break; }
     }
-    if (on) return 1u;
-  }
-  return 0u;
+    bit = on;
+    return on != 0;
+  });
+  return bit;
 }
 
 // patch NW consecutive match words v[] of message m, the first at local word wd0: one binary search for
@@ -432,72 +439,31 @@ __device__ __forceinline__ void apply_events(const DevState& s, const BatchIn& b
   }
 }
 
-// match word `wd` of a MSGF_TARGET message m (pcdn_send_to_broker(s)): the shard's broker mask for "every peer
-// broker", else the bit of its one target connection (0 when that connection lies outside this shard's slice).
-// No topic rows, in-batch events or to_users_only: the recipients are the brokers connected when it was sent.
-__device__ __forceinline__ uint32_t target_word(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd) {
-  const uint32_t c = b.aux_off[m];
-  if (c == kConnNone) return s.brk[wd];
-  const uint32_t local = c - s.conn_base;   // (unsigned wrap: below the base → outside the slice)
-  return local < s.N && (local >> 5) == wd ? 1u << (local & 31u) : 0u;
+// the batch's first kernel zeroes its counters (zero: null when a memset or an earlier kernel did); nothing else
+// in that kernel's first CTA touches them before its next barrier
+__device__ __forceinline__ void zero_stats(BatchStats* zero, bool first_cta) {
+  if (zero && first_cta && threadIdx.x < sizeof(BatchStats) / 4) reinterpret_cast<uint32_t*>(zero)[threadIdx.x] = 0;
 }
 
-// match word `wd` (32 connections) of message m: OR of its topics' bitmap rows (a2)
-// (TARGET: the batch holds a MSGF_TARGET message; only that instantiation reads the flag)
-template <bool TARGET>
-__device__ __forceinline__ uint32_t match_word(const DevState& s, const BatchIn& b, uint32_t m, uint32_t wd) {
-  const uint32_t toff = b.aux_off[m], tn = b.aux_len[m];
-  const uint32_t fl = b.flags[m];
-  if (TARGET && (fl & MSGF_TARGET)) return target_word(s, b, m, wd);
-  uint32_t word = 0;
-  if (fl & MSGF_TOPICS_U8) {  // wire topic list read in place (device-parse mode)
-    const uint8_t* tb = b.arena + toff;
-    for (uint32_t i = 0; i < tn; i++) {
-      if ((fl & MSGF_PRUNE) && !topic_kept(tb, i, s.n_valid_topics)) continue;
-      const uint32_t t = tb[i];
-      if (t < s.T) word |= s.sub[(size_t)t * s.W + wd];
-    }
-  } else {
-    for (uint32_t i = 0; i < tn; i++) {
-      const uint32_t t = b.topics[toff + i];
-      if (t < s.T) word |= s.sub[(size_t)t * s.W + wd];
-    }
-  }
-  if (b.n_events) apply_events<1>(s, b, m, wd, &word);
-  if (fl & MSGF_USERS_ONLY) word &= ~s.brk[wd];  // to_users_only (connections/mod.rs:111)
-  return word;
-}
-// Warp = one 256-word match block of one message, lane = 8 consecutive words (32-byte vector
+// Warp = one 256-word match block `blk` of broadcast j, lane = 8 consecutive words (32-byte vector
 // loads of the bitmap rows, no block-level synchronisation: the popcount prefix of a 256-word block
-// is a lane-local prefix plus one warp scan).  grid = (ceil(nblk / 8), n_bcast).
+// is a lane-local prefix plus one warp scan).  Run by k_match and by the fused small-engine kernel.
+// (EVENTS: the batch holds in-batch subscription events; TARGET: it holds a MSGF_TARGET message, and only
+//  that instantiation reads the flag)
 template <bool EVENTS, bool TARGET>
-__global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, BatchStats* zero) {
-  // the batch's first kernel when it has no direct message and no device parse: it zeroes the counters
-  // (nothing else in this launch touches them) instead of a memset on the stream
-  if (zero && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x < sizeof(BatchStats) / 4) reinterpret_cast<uint32_t*>(zero)[threadIdx.x] = 0;
-  const uint32_t j = blockIdx.y, lane = lane_id();
-  const uint32_t blk = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (blk >= s.nblk) return;  // warp-uniform
+__device__ __forceinline__ void match_block(const DevState& s, const BatchIn& b, const Work& w, uint32_t j, uint32_t blk) {
+  const uint32_t lane = lane_id();
   const uint32_t m = b.bcast_index[j];
   const uint32_t w0 = blk * kBlockWords + lane * 8;
-  const uint32_t toff = b.aux_off[m], tn = b.aux_len[m], fl = b.flags[m];
+  const uint32_t toff = b.aux_off[m], fl = b.flags[m];
   uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, 0);
-  auto or_row = [&](uint32_t t) {
-    if (t >= s.T) return;
+  for_each_topic(s, b, fl, toff, b.aux_len[m], [&](uint32_t t) {   // OR of the topics' bitmap rows
     const uint4* row = reinterpret_cast<const uint4*>(s.sub + (size_t)t * s.W + w0);
     const uint4 a = row[0], c = row[1];
     lo.x |= a.x; lo.y |= a.y; lo.z |= a.z; lo.w |= a.w;
     hi.x |= c.x; hi.y |= c.y; hi.z |= c.z; hi.w |= c.w;
-  };
-  if (fl & MSGF_TOPICS_U8) {  // wire topic list read in place (device-parse mode)
-    const uint8_t* tb = b.arena + toff;
-    for (uint32_t i = 0; i < tn; i++) {
-      if ((fl & MSGF_PRUNE) && !topic_kept(tb, i, s.n_valid_topics)) continue;
-      or_row(tb[i]);
-    }
-  } else {
-    for (uint32_t i = 0; i < tn; i++) or_row(b.topics[toff + i]);
-  }
+    return false;
+  });
   if (EVENTS && !(TARGET && (fl & MSGF_TARGET))) {
     uint32_t v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
     apply_events<8>(s, b, m, w0, v);
@@ -509,7 +475,9 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, Ba
     lo.x &= ~a.x; lo.y &= ~a.y; lo.z &= ~a.z; lo.w &= ~a.w;
     hi.x &= ~c.x; hi.y &= ~c.y; hi.z &= ~c.z; hi.w &= ~c.w;
   }
-  // pcdn_send_to_broker(s): the target's row (target_word, eight words at once).  A MSGF_TARGET message lists no
+  // pcdn_send_to_broker(s): the row is the shard's broker mask for "every peer broker", else the bit of the one
+  // target connection (none when it lies outside this shard's slice).  No topic rows, in-batch events or
+  // to_users_only: the recipients are the brokers connected when it was sent.  A MSGF_TARGET message lists no
   // topic and is never to_users_only, so lo / hi are still zero here.
   if (TARGET && (fl & MSGF_TARGET)) {
     if (toff == kConnNone) {
@@ -552,6 +520,14 @@ __global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, Ba
     }
     if (lane == 0) { w.D[m] = carry; w.jidx[m] = j; w.done[j] = 0; }
   }
+}
+// grid = (ceil(nblk / 8), n_bcast); zero: see zero_stats (the batch's first kernel when it has no direct message
+// and no device parse)
+template <bool EVENTS, bool TARGET>
+__global__ void __launch_bounds__(256) k_match(DevState s, BatchIn b, Work w, BatchStats* zero) {
+  zero_stats(zero, blockIdx.x == 0 && blockIdx.y == 0);
+  const uint32_t blk = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (blk < s.nblk) match_block<EVENTS, TARGET>(s, b, w, blockIdx.y, blk);  // warp-uniform
 }
 void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, bool targeted, cudaStream_t st) {
   if (!b.n_bcast) return;
@@ -607,36 +583,50 @@ __device__ __forceinline__ void plan_classify(const DevState& s, const BatchIn& 
   *cls_out = cls; *tiles_out = tiles;
 }
 
-__global__ void __launch_bounds__(256) k_plan_a(DevState s, BatchIn b, Work w, uint32_t nblk) {
-  __shared__ uint32_t sm[9];
-  const uint32_t m = blockIdx.x * 256 + threadIdx.x;
+// Thread per message m of CTA vb of nvb (NW warps each): class, tiles, and the four CTA-local exclusive scans —
+// fat entries, thin entries, tiles, connection-major rank — stored per message; thread 0 stores the CTA's totals
+// into scan_tmp.  Returns m's connection-major rank; *cm: m is connection-major.
+template <int NW>
+__device__ __forceinline__ uint32_t plan_messages(const DevState& s, const BatchIn& b, const Work& w, uint32_t m, uint32_t vb,
+                                                  uint32_t nvb, uint32_t* sm, bool* cm) {
   const bool valid = m < b.n_msgs;
   const uint32_t d = valid ? w.D[m] : 0;
   uint32_t cls, tiles;
   plan_classify(s, b, m, d, &cls, &tiles);
   uint32_t tot;
-  uint32_t e0 = block256_excl_scan(cls != CLS_THIN ? d : 0, &tot, sm);
-  if (threadIdx.x == 0) w.scan_tmp[blockIdx.x] = tot;
-  uint32_t e1 = block256_excl_scan(cls == CLS_THIN ? d : 0, &tot, sm);
-  if (threadIdx.x == 0) w.scan_tmp[nblk + blockIdx.x] = tot;
-  uint32_t e2 = block256_excl_scan(tiles, &tot, sm);
-  if (threadIdx.x == 0) w.scan_tmp[2 * nblk + blockIdx.x] = tot;
-  uint32_t e3 = block256_excl_scan(cls == CLS_CM ? 1u : 0u, &tot, sm);
-  if (threadIdx.x == 0) w.scan_tmp[3 * nblk + blockIdx.x] = tot;
+  uint32_t e0 = cta_excl_scan<NW>(cls != CLS_THIN ? d : 0, &tot, sm);
+  if (threadIdx.x == 0) w.scan_tmp[vb] = tot;
+  uint32_t e1 = cta_excl_scan<NW>(cls == CLS_THIN ? d : 0, &tot, sm);
+  if (threadIdx.x == 0) w.scan_tmp[nvb + vb] = tot;
+  uint32_t e2 = cta_excl_scan<NW>(tiles, &tot, sm);
+  if (threadIdx.x == 0) w.scan_tmp[2 * nvb + vb] = tot;
+  uint32_t e3 = cta_excl_scan<NW>(cls == CLS_CM ? 1u : 0u, &tot, sm);
+  if (threadIdx.x == 0) w.scan_tmp[3 * nvb + vb] = tot;
   if (valid) { w.eb_fat[m] = e0; w.eb_thin[m] = e1; w.tbase[m] = e2; w.cm_rank[m] = e3; w.cls[m] = (uint8_t)cls; }
-  if (gridDim.x == 1) {
-    // whole batch in one block (<= 256 messages): the local scans are already global, finish here
-    // (saves the k_plan_b / k_plan_c launches on the latency-critical small-batch path)
-    if (valid && cls == CLS_CM) w.cm_list[e3] = m;
-    if (threadIdx.x == 0) {
-      const uint32_t t0 = w.scan_tmp[0], t1 = w.scan_tmp[1], t2 = w.scan_tmp[2], t3 = w.scan_tmp[3];
-      w.stats->n_fat_entries = t0; w.stats->n_thin_entries = t1; w.stats->n_fat_tiles = t2; w.stats->tile_cursor = 0;
-      w.stats->n_cm = t3; w.stats->cm_cursor = 0;
-      if (t0 > w.cap_fat || t1 > w.cap_thin) w.stats->status = 1;  // PCDN_E2BIG
-      const uint32_t n = b.n_msgs;
-      w.eb_fat[n] = t0; w.eb_thin[n] = t1; w.tbase[n] = t2; w.cm_rank[n] = t3;
-    }
+  *cm = valid && cls == CLS_CM;
+  return e3;
+}
+// Whole batch in one CTA (<= 256 messages): its scans are already global, so the plan ends here — cm_list,
+// the totals and cursors, the PCDN_E2BIG check and the [n] sentinels (what k_plan_b / k_plan_c do otherwise)
+__device__ __forceinline__ void plan_finish(const BatchIn& b, const Work& w, uint32_t m, bool cm, uint32_t cm_rank) {
+  if (cm) w.cm_list[cm_rank] = m;
+  if (threadIdx.x == 0) {
+    const uint32_t t0 = w.scan_tmp[0], t1 = w.scan_tmp[1], t2 = w.scan_tmp[2], t3 = w.scan_tmp[3];
+    w.stats->n_fat_entries = t0; w.stats->n_thin_entries = t1; w.stats->n_fat_tiles = t2; w.stats->tile_cursor = 0;
+    w.stats->n_cm = t3; w.stats->cm_cursor = 0;
+    if (t0 > w.cap_fat || t1 > w.cap_thin) w.stats->status = 1;  // PCDN_E2BIG
+    const uint32_t n = b.n_msgs;
+    w.eb_fat[n] = t0; w.eb_thin[n] = t1; w.tbase[n] = t2; w.cm_rank[n] = t3;
   }
+}
+
+__global__ void __launch_bounds__(256) k_plan_a(DevState s, BatchIn b, Work w, uint32_t nblk) {
+  __shared__ uint32_t sm[9];
+  const uint32_t m = blockIdx.x * 256 + threadIdx.x;
+  bool cm;
+  const uint32_t r = plan_messages<8>(s, b, w, m, blockIdx.x, nblk, sm, &cm);
+  // (one block: saves the k_plan_b / k_plan_c launches on the latency-critical small-batch path)
+  if (gridDim.x == 1) plan_finish(b, w, m, cm, r);
 }
 // grid = 4: block q scans the block totals of one of the four planned quantities
 __global__ void __launch_bounds__(256) k_plan_b(Work w, uint32_t nblk) {
@@ -716,7 +706,6 @@ __device__ __forceinline__ uint32_t alloc_record(ConnCursor& k, uint32_t u, uint
 // deterministic rank (block base + word prefix + lane rank).
 // (body shared by k_offsets — 256-thread CTAs, any N — and the fused small-engine control kernel —
 //  eight 1024-thread CTAs of one cluster, N = 8192; NT = threads per CTA, c = this thread's connection)
-// SPARSE_BOUNDS: the fused small-engine kernel's direct segments (rank-sorted, bounds valid iff stamped)
 // Pool mode (DevState::pool): the CTAs of the offsets pass chain their unit totals in connection order
 // with a decoupled look-back (one 64-bit word per CTA: batch stamp | flag | value, so nothing is
 // cleared between batches).  Called by warp 0 of the CTA; returns the units of all CTAs before `vb`.
@@ -776,11 +765,12 @@ __device__ __forceinline__ void pool_allocate(const DevState& s, const Work& w, 
   bs->pool_base = base; bs->pool_units = total; bs->pool_skip = skip;
 }
 
-// Pool mode, two ways to chain the CTAs' unit totals: LOOKBACK (the fused small-engine kernel: its CTAs
-// are co-resident, the chain is at most 64 long) or, in the regular kernel, CTA-local offsets + the
-// CTA total in lb_tot[], finished by k_pool_finish (one more launch instead of 4096 CTAs polling each
-// other is slower at 2^20 connections).
-template <bool HAS_DIRECT, int NT, bool SPARSE_BOUNDS, bool LOOKBACK>
+// FUSED: run by the fused small-engine kernel.  Its direct segments are rank-sorted with sparse bounds (valid
+// iff stamped), and in pool mode its CTAs chain their unit totals with a look-back (they are co-resident, the
+// chain is at most 64 long).  The regular kernel's CTAs instead keep CTA-local offsets and put the CTA total
+// in lb_tot[], finished by k_pool_finish (one more launch instead of 4096 CTAs polling each other is slower
+// at 2^20 connections).
+template <bool HAS_DIRECT, int NT, bool FUSED>
 __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b, const Work& w, uint32_t max_conns,
                                              uint32_t c, uint32_t vb, uint32_t nvb) {
   constexpr int NW = NT / 32;
@@ -795,7 +785,7 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
   k.s1_off = 0; k.s1_units = 0; k.s1_rec = 0; k.s2_units = 0; k.s2_rec = 0; k.ovf = 0; k.in2 = 0; k.bytes = 0;
   uint32_t dp = 0, de = 0;
   if (HAS_DIRECT) {
-    if (SPARSE_BOUNDS) {
+    if (FUSED) {
       if (w.dstamp[c] == w.stamp) { dp = w.dstart[c]; de = w.dend[c]; }
     } else {
       dp = dseg_start(w, c); de = dseg_start(w, c + 1);
@@ -905,7 +895,7 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
     __shared__ uint32_t cta_prefix;
     uint32_t ctot;
     const uint32_t cex = cta_excl_scan<NW>(k.bu, &ctot, sm);
-    if (LOOKBACK) {
+    if (FUSED) {
       if (threadIdx.x < 32) {
         const uint32_t pre = pool_lookback(w, vb, ctot);
         if (threadIdx.x == 0) {
@@ -992,7 +982,7 @@ __device__ __forceinline__ void offsets_body(const DevState& s, const BatchIn& b
 }
 template <bool HAS_DIRECT>
 __global__ void __launch_bounds__(256) k_offsets(DevState s, BatchIn b, Work w, uint32_t max_conns) {
-  offsets_body<HAS_DIRECT, 256, false, false>(s, b, w, max_conns, blockIdx.x * 256 + threadIdx.x, blockIdx.x, gridDim.x);  // N is a multiple of 8192
+  offsets_body<HAS_DIRECT, 256, false>(s, b, w, max_conns, blockIdx.x * 256 + threadIdx.x, blockIdx.x, gridDim.x);  // N is a multiple of 8192
 }
 // Pool mode, after k_offsets: every CTA scans the (at most a few thousand) CTA totals in shared memory
 // — redundantly, 16 KB of reads each, cheaper than a second dependent launch — then the grid adds each
@@ -1043,21 +1033,23 @@ void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has
 // hundred to a few thousand consensus nodes, one vote or proposal at a time).  There the regular pipeline is a chain of five
 // tiny dependent launches; here match, plan and offsets run in ONE launch on one cluster of eight
 // 1024-thread CTAs — a thread per connection and 8192-connection pass — with cluster barriers where the pipeline has kernel
-// boundaries.  It writes exactly the arrays k_match / k_plan_a / k_offsets write (the
-// pack kernel and the host cannot tell the difference), zeroes the batch counters itself when no
-// earlier kernel of the batch needs them, and publishes the final counters into mapped host memory.
+// boundaries.  It runs the code of k_match (match_block), k_plan_a (plan_messages, plan_finish) and
+// k_offsets (offsets_body), so it writes exactly the arrays they write (the pack kernel and the host
+// cannot tell the difference), zeroes the batch counters itself when no earlier kernel of the batch
+// needs them, and publishes the final counters into mapped host memory.
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// one warp per match item: the whole match of a batch the fused path takes is one pass of the cluster's warps
+static_assert(kSmallCtrlItems == 8 * 1024 / 32, "kSmallCtrlItems = the warps of k_ctrl_small's 8 CTAs of 1024 threads");
 // offsets_only: the retry of a batch the output pool refused — the routing of the first run (direct
 // bounds, match words, plan) is still in the scratch, only the offsets pass runs again.
 template <bool HAS_DIRECT, bool TARGET>
 __global__ void __cluster_dims__(8, 1, 1) __launch_bounds__(1024, 1)
-k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish, int offsets_only) {
+k_ctrl_small(DevState s, BatchIn b, Work w, BatchStats* zero, BatchStats* publish, int offsets_only) {
   __shared__ uint32_t sm[33];
-  __shared__ uint32_t gbase[5];
   const uint32_t tid = threadIdx.x, rank = blockIdx.x;  // grid = one cluster
-  if (zero_stats && rank == 0 && tid < sizeof(BatchStats) / 4) reinterpret_cast<uint32_t*>(w.stats)[tid] = 0;
+  zero_stats(zero, rank == 0);
 
   // ---- direct messages (= k_direct_lookup + the grouping by connection) on CTA 0; at most
   //      kSmallCtrlMsgs of them, so the (connection, message) order is a rank count
@@ -1084,67 +1076,22 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish,
     }
   }
 
-  // ---- match (= k_match): four (message, 256-word block) items per pass and CTA
+  // ---- match (= k_match): warp = one (broadcast, 256-word block) item, the last warp of a broadcast
+  //      writes its block bases and D_m
   if (!offsets_only) {
-    const uint32_t q = tid >> 8, wl = tid & 255u, nitems = b.n_bcast * s.nblk;
-    for (uint32_t i0 = rank * 4; i0 < nitems; i0 += 32) {  // trip count is uniform inside a CTA
-      const uint32_t it = i0 + q;
-      const bool live = it < nitems;
-      const uint32_t j = live ? it / s.nblk : 0, blk = live ? it % s.nblk : 0;
-      const uint32_t wd = blk * kBlockWords + wl;
-      const uint32_t word = live ? match_word<TARGET>(s, b, b.bcast_index[j], wd) : 0;
-      uint32_t tot, ex = cta_excl_scan<32>(__popc(word), &tot, sm);
-      if (wl == 0) gbase[q] = ex;
-      if (tid == 0) gbase[4] = tot;
-      __syncthreads();
-      if (live) {
-        w.B[(size_t)j * s.W + wd] = word;
-        w.wpre[(size_t)j * s.W + wd] = (uint16_t)(ex - gbase[q]);
-        if (wl == 0) w.cnt[(size_t)j * s.nblk + blk] = gbase[q + 1] - gbase[q];
-      }
-      __syncthreads();
+    const uint32_t item = rank * 32 + (tid >> 5), nblk = s.nblk;
+    if (item < b.n_bcast * nblk) {   // warp-uniform
+      if (b.n_events) match_block<true, TARGET>(s, b, w, item / nblk, item % nblk);
+      else match_block<false, TARGET>(s, b, w, item / nblk, item % nblk);
     }
   }
   cluster_sync_all();
 
-  // ---- block bases and D_m of every broadcast (thread = message; at most 8 blocks each) on CTA 0
+  // ---- plan (= k_plan_a of a one-block batch) on CTA 0
   if (rank == 0 && !offsets_only) {
-    if (tid < b.n_bcast) {
-      uint32_t carry = 0;
-      for (uint32_t blk = 0; blk < s.nblk; blk++) {
-        const uint32_t v = w.cnt[(size_t)tid * s.nblk + blk];
-        w.base[(size_t)tid * s.nblk + blk] = carry;
-        carry += v;
-      }
-      const uint32_t m = b.bcast_index[tid];
-      w.D[m] = carry; w.jidx[m] = tid;
-    }
-    __syncthreads();
-  }
-
-  // ---- plan (= the single-block case of k_plan_a) on CTA 0
-  if (rank == 0 && !offsets_only) {
-    const uint32_t m = tid;
-    const bool valid = m < b.n_msgs;
-    const uint32_t d = valid ? w.D[m] : 0;
-    uint32_t cls, tiles;
-    plan_classify(s, b, m, d, &cls, &tiles);
-    uint32_t t0, t1, t2, t3;
-    const uint32_t e0 = cta_excl_scan<32>(cls != CLS_THIN ? d : 0, &t0, sm);
-    const uint32_t e1 = cta_excl_scan<32>(cls == CLS_THIN ? d : 0, &t1, sm);
-    const uint32_t e2 = cta_excl_scan<32>(tiles, &t2, sm);
-    const uint32_t e3 = cta_excl_scan<32>(cls == CLS_CM ? 1u : 0u, &t3, sm);
-    if (valid) {
-      w.eb_fat[m] = e0; w.eb_thin[m] = e1; w.tbase[m] = e2; w.cm_rank[m] = e3; w.cls[m] = (uint8_t)cls;
-      if (cls == CLS_CM) w.cm_list[e3] = m;
-    }
-    if (tid == 0) {
-      w.stats->n_fat_entries = t0; w.stats->n_thin_entries = t1; w.stats->n_fat_tiles = t2; w.stats->tile_cursor = 0;
-      w.stats->n_cm = t3; w.stats->cm_cursor = 0;
-      if (t0 > w.cap_fat || t1 > w.cap_thin) w.stats->status = 1;  // PCDN_E2BIG
-      const uint32_t n = b.n_msgs;
-      w.eb_fat[n] = t0; w.eb_thin[n] = t1; w.tbase[n] = t2; w.cm_rank[n] = t3;
-    }
+    bool cm;
+    const uint32_t r = plan_messages<32>(s, b, w, tid, 0, 1, sm, &cm);
+    plan_finish(b, w, tid, cm, r);
   }
   cluster_sync_all();
 
@@ -1153,7 +1100,7 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish,
   //  cluster are co-resident and earlier passes are complete, so the look-back never waits on a CTA
   //  that has not started)
   for (uint32_t c0 = 0; c0 < s.N; c0 += 8192)
-    offsets_body<HAS_DIRECT, 1024, true, true>(s, b, w, s.N, c0 + rank * 1024 + tid, c0 / 1024 + rank, s.N / 1024);
+    offsets_body<HAS_DIRECT, 1024, true>(s, b, w, s.N, c0 + rank * 1024 + tid, c0 / 1024 + rank, s.N / 1024);
 
   // ---- final counters straight into the host's (mapped, pinned) result block
   if (publish) {
@@ -1162,15 +1109,15 @@ k_ctrl_small(DevState s, BatchIn b, Work w, int zero_stats, BatchStats* publish,
       reinterpret_cast<uint32_t*>(publish)[tid] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + tid);
   }
 }
-void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, bool zero_stats,
+void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, BatchStats* zero,
                        BatchStats* publish, bool offsets_only, cudaStream_t st) {
-  const int z = zero_stats ? 1 : 0, oo = offsets_only ? 1 : 0;
+  const int oo = offsets_only ? 1 : 0;
   if (targeted) {   // (as in launch_match: the instantiations without target rows stay as they are)
-    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, true><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
-    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, true><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, true><<<8, 1024, 0, st>>>(s, b, w, zero, publish, oo);
+    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, true><<<8, 1024, 0, st>>>(s, b, w, zero, publish, oo);
   } else {
-    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, false><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
-    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, false><<<8, 1024, 0, st>>>(s, b, w, z, publish, oo);
+    if (has_direct) PCDN_COUNT_LAUNCH, k_ctrl_small<true, false><<<8, 1024, 0, st>>>(s, b, w, zero, publish, oo);
+    else PCDN_COUNT_LAUNCH, k_ctrl_small<false, false><<<8, 1024, 0, st>>>(s, b, w, zero, publish, oo);
   }
 }
 

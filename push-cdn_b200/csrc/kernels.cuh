@@ -244,16 +244,17 @@ struct UpdSlot { uint32_t slot; CuckooEntry e; };
 void launch_apply_updates(const DevState& s, const Upd32* u32, uint32_t n32, const UpdSlot* us,
                           uint32_t nslot, const uint32_t* key_slots, const uint8_t* key_bytes,
                           uint32_t nkeys, cudaStream_t st);
-void launch_batch_begin(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, cudaStream_t st);
+void launch_batch_begin(const Work& w, cudaStream_t st);
 void launch_parse(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st);
-// zero: the batch's counters, zeroed by k_match before any kernel writes one (null: zeroed earlier)
+// zero: the batch's counters, zeroed by k_match / k_ctrl_small before any kernel writes one (null: zeroed earlier)
 // targeted: the batch holds a MSGF_TARGET message (host-staged batches only)
 void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, bool targeted, cudaStream_t st);
 void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_offsets(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, int n_sms, cudaStream_t st);
-// fused match + plan + offsets for N <= kSmallCtrlConns and n_msgs <= kSmallCtrlMsgs (one cluster launch)
-void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, bool zero_stats,
+// fused match + plan + offsets for N <= kSmallCtrlConns, n_msgs <= kSmallCtrlMsgs and at most kSmallCtrlItems
+// match items (one cluster launch)
+void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, BatchStats* zero,
                        BatchStats* publish, bool offsets_only, cudaStream_t st);
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);

@@ -109,23 +109,41 @@ def test_connect_flow(pcdn, layout, flow):
     w.e.close()
 
 
-@pytest.mark.parametrize("control", ["fused", "regular-conns", "regular-msgs"])
+@pytest.mark.parametrize("control", ["fused", "fused-full", "regular-conns", "regular-msgs"])
 def test_control_paths(pcdn, control):
-    """fused k_ctrl_small; k_match on an engine with more than kSmallCtrlConns slots; k_match for a batch of
-    more than kSmallCtrlMsgs messages"""
+    """fused k_ctrl_small; the same with kSmallCtrlItems (broadcast, 8192-connection block) match items, one per
+    warp of the kernel, and in-batch subscription events of users on both match blocks and of a broker between
+    the sends; k_match on an engine with more than kSmallCtrlConns slots; k_match for a batch of more than
+    kSmallCtrlMsgs messages"""
+    block = K.kBlockWords * 32
     cfg = dict(max_conns=1024)
     if control == "regular-conns":
         cfg = dict(max_conns=K.kSmallCtrlConns * 2, ring_bytes_per_conn=1 << 14, max_keys=1 << 17)
+    if control == "fused-full":
+        cfg = dict(max_conns=2 * block, ring_bytes_per_conn=1 << 17, flags=pcdn.FLAG_INBATCH_SUBSCRIBE)
     w = SendWorld(pcdn, **cfg)
     rng = random.Random(3)
-    populate(w)
+    n_users = block + 200 if control == "fused-full" else 200
+    populate(w, n_users)
     n = K.kSmallCtrlMsgs + 20 if control == "regular-msgs" else 30
+    if control == "fused-full":
+        nblk = -(-w.e.shard_info(0).shard_stride // block)
+        assert nblk == 2
+        n = K.kSmallCtrlItems // nblk
+    edges = [0, 31, 32, block - 1, block, block + 1, n_users - 1]
+    b0 = w.e.stats().batches
     for j in range(n):
+        if control == "fused-full" and j % 5 == 2:
+            sub = j % 2
+            w.both("subscribe_user_to" if sub else "unsubscribe_user_from", b"user-%05d" % edges[j % len(edges)], [(j + 1) % 4])
+            w.both("subscribe_broker_to" if sub else "unsubscribe_broker_from", "b/b", [j % 4])
         if j % 7 == 3:
             assert w.send("b/b" if j % 2 else None, user_sync(j, rng.randint(1, 2000))) == 0
         else:
             w.bcast([j % 4], orc.broadcast_frame([j % 4], payload(rng, rng.randint(1, 600))))
     assert w.check() > 0
+    if control == "fused-full":
+        assert w.e.stats().batches == b0 + 1
     w.e.close()
 
 
