@@ -164,27 +164,24 @@ BatchIn bind_batch(const uint8_t* arena, const uint8_t* desc, const DescLayout& 
 // and run much longer; the overlap hides at most the short control stage, so it stops paying for long packs.
 static constexpr unsigned long long kOverlapMaxBytes = 3ull << 29;
 
-// run the kernel pipeline of one shard for slot `si`, whose BatchIn is ready (or will be, once
-// ev_ingest fires) in that shard's memory.
-// retry (output pool): the slot holds a batch the pool refused.  Its routing (parse, direct lookup,
-// match, plan: everything that reads the tables) is kept as it was computed at launch; only the passes
-// that place it in the pool and pack it run again: offsets (+ pool finish) and pack.
-int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_direct, bool devparse, bool wait_ingest, bool retry = false) {
-  DeviceGuard dg(sh.device);
+// Who zeroes a batch's counters (BatchStats): the first CTA of its first kernel, k_ctrl_small or k_match, unless k_parse
+// or the regular direct lookup counts into them first from many CTAs, or no k_match runs: then a memset.  A retry zeroes
+// nothing: the counters keep the plan's totals, and k_pool_retry_begin resets what offsets and pack count.
+enum : uint8_t { ZERO_NONE, ZERO_MEMSET, ZERO_MATCH, ZERO_CTRL_SMALL };
+uint8_t counters_zeroer(const Slot& hs, const BatchIn& in, bool fused, bool retry) {
+  if (retry) return ZERO_NONE;
+  if (hs.devparse || (!fused && (hs.n_direct || !in.n_bcast))) return ZERO_MEMSET;
+  return fused ? ZERO_CTRL_SMALL : ZERO_MATCH;
+}
+
+// begin: the pack-stream prediction, the ingest wait, the launch's stamp and batch id, the span path
+int batch_begin(pcdn_engine* e, Shard& sh, uint32_t si, bool fused, bool wait_ingest, bool retry) {
   ShardSlot& s = sh.slots[si];
-  // Default: the pack runs on the main stream.  On the high-priority pack stream the next batch's control
-  // kernels overlap it, which is slower for a long bulk-store pack; so only the batches below take it.
-  const bool dp = sh.direct_publish;
-  // Batches of nothing but many direct messages DO take the pack stream: their control kernels are
-  // latency-bound (three dependent random reads per message), their pack is a separate bandwidth-bound
-  // launch, and the two overlap well (config C4).
-  const bool direct_only = s.in.n_bcast == 0 && n_direct >= kThinSeparateMin;
-  // Broadcast batches: running the next batch's control stage beside this batch's pack helps when the pack is
-  // short and message-major (sparse fan-out, config 5) and hurts a long pack, which then shares SMs and HBM with
-  // it (config 5 dense, C2).  Which
-  // one this batch will be is decided on the device, so the class mix and size of the most recent COMPLETED batch
-  // of this shard predict it (a workload changes its mix rarely; a wrong guess costs one batch a few percent).
-  if (!dp && s.in.n_bcast > 0) {
+  // Broadcast batches: running the next batch's control stage beside this batch's pack helps when the pack is short
+  // and message-major (sparse fan-out, config 5) and hurts a long pack, which then shares SMs and HBM with it (config
+  // 5 dense, C2).  Which one this batch will be is decided on the device, so the class mix and size of the most recent
+  // COMPLETED batch of this shard predict it (a workload changes its mix rarely; a wrong guess costs a few percent).
+  if (!sh.direct_publish && s.in.n_bcast > 0) {
     for (int k = 0; k < 2; k++) {
       const int pv = sh.prev_slot[k];
       if (pv < 0 || pv == (int)si) continue;
@@ -196,63 +193,64 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
       break;
     }
   }
-  const bool fat_overlap = s.in.n_bcast > 0 && sh.fat_only;
-  sh.prev_slot[1] = sh.prev_slot[0];
-  sh.prev_slot[0] = (int)si;
-  cudaStream_t st = sh.stream, ps = (!dp && (direct_only || fat_overlap)) ? sh.pack_stream : sh.stream, cs = sh.copy_stream;
-  const bool has_direct = n_direct > 0;
-  const Slot& hs = e->slots[si];
-  if (wait_ingest) CUDA_TRY(cudaStreamWaitEvent(st, s.ev_ingest, 0));
-  s.timed = e->timing;
-  s.polled = false;
-  s.n_msg_errors = 0;
-  // validity stamp of this batch's direct buckets / look-back words (a retry keeps it: the fused
-  // kernel's direct bounds of the first run are valid under it)
+  sh.prev_slot[1] = sh.prev_slot[0]; sh.prev_slot[0] = (int)si;
+  if (wait_ingest) CUDA_TRY(cudaStreamWaitEvent(sh.stream, s.ev_ingest, 0));
+  s.timed = e->timing; s.polled = false; s.n_msg_errors = 0;
+  // validity stamp of the batch's direct buckets / look-back words (a retry keeps it: its direct bounds stay valid)
   if (!retry && ++s.w.stamp == 0) s.w.stamp = 1;
   if (!retry && sh.dev.pool && (s.w.stamp & 0x3FFFFFFFu) == 0) {   // the look-back words carry 30 bits of it
     s.w.stamp++;
-    CUDA_TRY(cudaMemsetAsync(s.w.lb_state, 0, ((size_t)sh.dev.N / 256 + 1) * 8, st));
+    CUDA_TRY(cudaMemsetAsync(s.w.lb_state, 0, ((size_t)sh.dev.N / 256 + 1) * 8, sh.stream));
   }
   s.w.pool_unblock = retry ? 1u : 0u;
   s.w.batch_id = retry ? e->slots[si].batch_id : e->next_batch_id;   // (launch_pipeline hands out next_batch_id)
-  // latency path of the smallest geometry: match + plan + offsets in one cluster launch that also
-  // zeroes / publishes the counters (kernels.cu: k_ctrl_small)
-  // (one cluster of 8 CTAs: worth it while the whole match is a few passes — a 128-message batch on a
-  //  65536-slot engine is 1024 (message, block) items and runs 10x faster through the regular kernels)
-  const bool fused = dp && sh.dev.N <= kSmallCtrlConns && s.in.n_msgs <= kSmallCtrlMsgs &&
-                     (uint64_t)s.in.n_bcast * sh.dev.nblk <= kSmallCtrlItems;
-  // Spans go straight into mapped host memory when few are expected (16-byte PCIe writes: a table
-  // of 16 K spans is slower than the staged copy): the smallest geometry, or a batch
-  // without broadcasts and with few messages (at most one span per message).  Otherwise they are staged in HBM and copied
-  // out with one DMA of the exact size while the pack runs.
-  s.spans_mapped = dp && (sh.dev.N <= 8192 || (s.in.n_bcast == 0 && s.in.n_msgs <= 4096));
+  // Spans go straight into mapped host memory when few are expected (16-byte PCIe writes: a table of 16 K spans is
+  // slower than the staged copy): the smallest geometry, or a batch without broadcasts and with few messages (at most
+  // one span per message).  Otherwise they are staged in HBM and copied out with one DMA of the exact size while the pack runs.
+  s.spans_mapped = sh.direct_publish && (sh.dev.N <= 8192 || (s.in.n_bcast == 0 && s.in.n_msgs <= 4096));
   if (sh.dev.pool && !fused) s.spans_mapped = false;   // k_pool_finish patches the table: keep it in HBM until it is final
   s.w.spans = s.spans_mapped ? s.d_spans_map : s.d_spans_dev;
   s.w.overflow = s.spans_mapped ? s.d_ovf_map : s.d_ovf_dev;
-  const bool zero_in_kernel = fused && !devparse && !retry;  // (k_parse counts into the batch counters before the fused kernel)
-  // regular pipeline: k_match zeroes the counters when it is the batch's first kernel (the direct lookup
-  // counts into them from many CTAs, and k_parse before it: those batches keep the memset)
-  const bool zero_in_match = !fused && !devparse && !retry && !has_direct && s.in.n_bcast > 0;
-  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[0], st));
+  if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[0], sh.stream));
+  return 0;
+}
+
+// control: route the batch (parse, direct lookup, match, plan: everything that reads the tables) and place it
+// (offsets).  retry: a batch the output pool refused keeps its routing; only the offsets (+ pool finish) run again.
+int batch_control(Shard& sh, ShardSlot& s, const Slot& hs, bool fused, bool retry) {
+  cudaStream_t st = sh.stream;
+  const uint8_t zero = counters_zeroer(hs, s.in, fused, retry);
   if (retry) {
     launch_pool_retry_begin(sh.dev, s.w, st);
   } else {
-    if (!zero_in_kernel && !zero_in_match) launch_batch_begin(s.w, st);
-    if (devparse) launch_parse(sh.dev, s.w, s.in, st);
-    if (has_direct && !fused) launch_direct(sh.dev, s.w, s.in, n_direct, st);  // fused: lookup + sort inside k_ctrl_small
+    if (zero == ZERO_MEMSET) CUDA_TRY(cudaMemsetAsync(s.w.stats, 0, sizeof(BatchStats), st));
+    if (hs.devparse) launch_parse(sh.dev, s.w, s.in, st);
+    if (hs.n_direct && !fused) launch_direct(sh.dev, s.w, s.in, hs.n_direct, st);  // fused: lookup + sort inside k_ctrl_small
   }
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[1], st));
   if (fused) {
-    launch_ctrl_small(sh.dev, s.w, s.in, has_direct, hs.targeted, zero_in_kernel ? s.w.stats : nullptr, s.d_stats_pub, retry, st);
+    launch_ctrl_small(sh.dev, s.w, s.in, hs.n_direct > 0, hs.targeted, zero == ZERO_CTRL_SMALL ? s.w.stats : nullptr, s.d_stats_pub, retry, st);
     if (s.timed) { CUDA_TRY(cudaEventRecord(s.ev[2], st)); CUDA_TRY(cudaEventRecord(s.ev[3], st)); }
   } else {
-    if (!retry) launch_match(sh.dev, s.w, s.in, zero_in_match ? s.w.stats : nullptr, hs.targeted, st);
+    if (!retry) launch_match(sh.dev, s.w, s.in, zero == ZERO_MATCH ? s.w.stats : nullptr, hs.targeted, st);
     if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[2], st));
     if (!retry) launch_plan(sh.dev, s.w, s.in, st);
-    launch_offsets(sh.dev, s.w, s.in, has_direct, sh.n_sms, st);   // pool mode: a pure function of the scratch
+    launch_offsets(sh.dev, s.w, s.in, hs.n_direct > 0, sh.n_sms, st);   // pool mode: a pure function of the scratch
     if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[3], st));
   }
-  if (!s.spans_mapped) {
+  return 0;
+}
+
+// pack: from the control stage's results to ev_done, which covers the batch's final counters in h_stats (published by
+// k_ctrl_small on the fused path, else by launch_pack)
+int batch_pack(pcdn_engine* e, Shard& sh, ShardSlot& s, const Slot& hs, bool fused) {
+  // Only two kinds of batch pack on the high-priority pack stream, beside the next batch's control kernels (which slow
+  // a long bulk-store pack): many direct messages alone, whose latency-bound lookup overlaps their bandwidth-bound pack
+  // well (config C4), and broadcasts batch_begin predicts to be short and message-major (sh.fat_only).
+  const bool fat_overlap = s.in.n_bcast > 0 && sh.fat_only;
+  const bool direct_only = s.in.n_bcast == 0 && hs.n_direct >= kThinSeparateMin;
+  cudaStream_t st = sh.stream, ps = (!sh.direct_publish && (direct_only || fat_overlap)) ? sh.pack_stream : st, cs = sh.copy_stream;
+  if (!s.spans_mapped) {   // (mapped spans: k_offsets wrote them to host memory; the host waits for ev_done only)
     CUDA_TRY(cudaEventRecord(s.ev_ctrl, st));
     // the span table is final once k_offsets is done: its counters go home while the pack runs
     CUDA_TRY(cudaStreamWaitEvent(cs, s.ev_ctrl, 0));
@@ -261,32 +259,39 @@ int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, uint32_t n_dir
     // pack on its own stream (packs of successive batches stay ordered among themselves)
     if (ps != st) CUDA_TRY(cudaStreamWaitEvent(ps, s.ev_ctrl, 0));
   }
-  // (mapped spans: k_offsets wrote spans / overflow into host memory; everything stays on one
-  //  stream and the host waits for ev_done only)
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[4], ps));
-  // k_pack CTAs per SM unless pack_variant bits 8-11 set them: 4 when the pack has the GPU to itself, 3 when it
-  // overlaps the next batch's control kernels (one H100: C2 +1.4 % with 4; the overlapped config-5 sparse shard
-  // +2 % with 3)
-  uint32_t pack_variant = e->cfg.pack_variant;
-  if (!((pack_variant >> 8) & 15u)) pack_variant |= (fat_overlap ? 3u : 4u) << 8;
-  // the final counters reach h_stats from the last pack kernel (mapped memory, covered by ev_done); only a
-  // batch without a pack launch copies them
+  // k_pack CTAs per SM unless pack_variant sets them: 4 when the pack has the GPU to itself, 3 when it overlaps the
+  // next batch's control kernels (one H100: C2 +1.4 % with 4; the overlapped config-5 sparse shard +2 % with 3)
+  const uint32_t pack_ctas = e->pack_ctas ? e->pack_ctas : fat_overlap ? 3u : 4u;
   // engines with ref_min_bytes: a host-staged batch runs k_pack_ref only when a message reaches the threshold; the
   // lengths of a device-resident batch are on the device, so it always does
   const bool has_ref = e->cfg.ref_min_bytes && (hs.device_input || hs.max_raw_len >= e->cfg.ref_min_bytes);
-  const bool published = launch_pack(sh.dev, s.w, s.in, n_direct, pack_variant, sh.n_sms, has_ref, fused ? nullptr : s.d_stats_pub, ps);
+  launch_pack(sh.dev, s.w, s.in, hs.n_direct, pack_ctas, e->direct_ctas, sh.n_sms, has_ref, fused ? nullptr : s.d_stats_pub, ps);
   if (s.timed) CUDA_TRY(cudaEventRecord(s.ev[5], ps));
   CUDA_TRY(cudaGetLastError());
-  if (!fused && !published) CUDA_TRY(cudaMemcpyAsync(s.h_stats, s.w.stats, sizeof(BatchStats), cudaMemcpyDeviceToHost, ps));
   CUDA_TRY(cudaEventRecord(s.ev_done, ps));
   return 0;
+}
+
+// the kernel pipeline of one shard for slot `si` (wait_ingest: its BatchIn is ready once ev_ingest fires; retry: see batch_control)
+int launch_shard_pipeline(pcdn_engine* e, Shard& sh, uint32_t si, bool wait_ingest, bool retry = false) {
+  DeviceGuard dg(sh.device);
+  ShardSlot& s = sh.slots[si];
+  // latency path of the smallest geometry: match + plan + offsets in one cluster launch (kernels.cu: k_ctrl_small)
+  // (one cluster of 8 CTAs: worth it while the whole match is a few passes — a 128-message batch on a
+  //  65536-slot engine is 1024 (message, block) items and runs 10x faster through the regular kernels)
+  const bool fused = sh.direct_publish && sh.dev.N <= kSmallCtrlConns && s.in.n_msgs <= kSmallCtrlMsgs &&
+                     (uint64_t)s.in.n_bcast * sh.dev.nblk <= kSmallCtrlItems;
+  if (int rc = batch_begin(e, sh, si, fused, wait_ingest, retry)) return rc;
+  if (int rc = batch_control(sh, s, e->slots[si], fused, retry)) return rc;
+  return batch_pack(e, sh, s, e->slots[si], fused);
 }
 
 // every local shard runs the pipeline on the open slot `si`; it becomes the newest in-flight batch
 int launch_pipeline(pcdn_engine* e, uint32_t si, bool wait_ingest) {
   Slot& s = e->slots[si];
   for (Shard& sh : e->shards) {
-    int rc = launch_shard_pipeline(e, sh, si, s.n_direct, s.devparse, wait_ingest);
+    int rc = launch_shard_pipeline(e, sh, si, wait_ingest);
     if (rc) return rc;
   }
   s.state = SLOT_INFLIGHT;
@@ -1157,6 +1162,8 @@ int pcdn_create(const pcdn_config* cfg, pcdn_engine** out) {
           return fail(PCDN_EINVAL, "PCDN_INGEST_NCCL needs one GPU per shard (use PCDN_INGEST_HOST for shards that share a device)");
   pcdn_engine* e = new pcdn_engine();
   e->cfg = *cfg;
+  e->pack_ctas = (cfg->pack_variant >> 8) & 15u;
+  if (const uint32_t d = (cfg->pack_variant >> 12) & 15u) e->direct_ctas = d;
   e->identity = cfg->identity ? cfg->identity : "/";
   e->cfg.identity = e->identity.c_str();
   e->world_shards = world;
@@ -1809,7 +1816,6 @@ int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id) {
   if (si < 0) return fail(PCDN_ENOENT, "unknown batch id");
   if (e->inflight.empty() || e->inflight.front() != batch_id)
     return fail(PCDN_EINVAL, "only the oldest unreleased batch can be retried (release the older ones first)");
-  Slot& s = e->slots[si];
   int rc = 0;
   uint32_t n = 0;
   for (Shard& sh : e->shards) {
@@ -1819,7 +1825,7 @@ int pcdn_retry_batch(pcdn_engine* e, uint64_t batch_id) {
       CUDA_TRY(cudaEventSynchronize(ss.ev_done));
     }
     if (ss.h_stats->status != 2) continue;   // this shard packed its share (or refused it for good): leave it alone
-    if ((rc = launch_shard_pipeline(e, sh, (uint32_t)si, s.n_direct, s.devparse, false, true))) return rc;
+    if ((rc = launch_shard_pipeline(e, sh, (uint32_t)si, false, true))) return rc;
     n++;
   }
   if (!n) return fail(PCDN_EINVAL, "the batch was not refused for space");

@@ -236,6 +236,8 @@ struct pcdn_engine {
   uint64_t pool_bytes = 0;        // PCDN_FLAG_OUTPUT_POOL: bytes of the output pool per shard
   std::vector<UpdSlot> h_slot; std::vector<uint32_t> h_kslot; std::vector<uint8_t> h_kbytes;  // journal parts common to all shards
   bool timing = false;
+  // pcdn_config.pack_variant: CTAs per SM of k_pack (0 = chosen per batch, batch_pack) and of k_pack_direct
+  uint32_t pack_ctas = 0, direct_ctas = 8;
   pcdn_message_hook hook[2] = {nullptr, nullptr};  // [origin]: MessageHookDef of user / broker connections
   void* hook_user[2] = {nullptr, nullptr};
   uint64_t inflight_bytes = 0;  // Limiter analogue: accepted frame bytes whose batch is not released yet

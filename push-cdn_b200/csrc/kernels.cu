@@ -355,10 +355,6 @@ __global__ void __launch_bounds__(256) k_dsort_hot(BatchIn b, Work w, uint32_t w
   }
 }
 
-void launch_batch_begin(const Work& w, cudaStream_t st) {
-  cudaMemsetAsync(w.stats, 0, sizeof(BatchStats), st);
-}
-
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st) {
   const uint32_t n = b.n_msgs;
   const uint32_t nseg = s.N + 1, ntiles = (nseg + 1023) / 1024;
@@ -443,6 +439,15 @@ __device__ __forceinline__ void apply_events(const DevState& s, const BatchIn& b
 // in that kernel's first CTA touches them before its next barrier
 __device__ __forceinline__ void zero_stats(BatchStats* zero, bool first_cta) {
   if (zero && first_cta && threadIdx.x < sizeof(BatchStats) / 4) reinterpret_cast<uint32_t*>(zero)[threadIdx.x] = 0;
+}
+// copy of the final counters into the mapped host block: fenced after publish_if_last's count of finished CTAs, not
+// after k_ctrl_small's cluster barrier (~0.8 us of its 15 us one-broadcast batch on an H100 80GB HBM3 at 700 W)
+__device__ __forceinline__ void publish_stats(const Work& w, BatchStats* publish, bool fenced) {
+  if (threadIdx.x < sizeof(BatchStats) / 4) {
+    if (fenced) __threadfence();
+    reinterpret_cast<uint32_t*>(publish)[threadIdx.x] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + threadIdx.x);
+    if (fenced) __threadfence_system();
+  }
 }
 
 // Warp = one 256-word match block `blk` of broadcast j, lane = 8 consecutive words (32-byte vector
@@ -1102,11 +1107,9 @@ k_ctrl_small(DevState s, BatchIn b, Work w, BatchStats* zero, BatchStats* publis
   for (uint32_t c0 = 0; c0 < s.N; c0 += 8192)
     offsets_body<HAS_DIRECT, 1024, true>(s, b, w, s.N, c0 + rank * 1024 + tid, c0 / 1024 + rank, s.N / 1024);
 
-  // ---- final counters straight into the host's (mapped, pinned) result block
-  if (publish) {
+  if (publish) {   // ---- final counters straight into the host's (mapped, pinned) result block
     cluster_sync_all();
-    if (rank == 0 && tid < sizeof(BatchStats) / 4)
-      reinterpret_cast<uint32_t*>(publish)[tid] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + tid);
+    if (rank == 0) publish_stats(w, publish, false);
   }
 }
 void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool has_direct, bool targeted, BatchStats* zero,
@@ -1396,7 +1399,7 @@ __device__ __forceinline__ void pack_direct_phase(const DevState& s, const Batch
   }
 }
 
-// The kernel that ends a batch publishes its final counters into mapped host memory, so that the batch's
+// The pack kernel that ends a batch publishes its final counters into mapped host memory, so that the batch's
 // ev_done covers them without a device-to-host copy on the stream between one pack and the next batch.
 // Every CTA counts itself done (also when the batch was refused); the last one copies the counters.
 __device__ __forceinline__ void publish_if_last(const Work& w, BatchStats* publish) {
@@ -1408,11 +1411,7 @@ __device__ __forceinline__ void publish_if_last(const Work& w, BatchStats* publi
     last = atomicAdd(&w.stats->ctas_done, 1u) == gridDim.x - 1 ? 1u : 0u;
   }
   __syncthreads();
-  if (last && threadIdx.x < sizeof(BatchStats) / 4) {
-    __threadfence();
-    reinterpret_cast<volatile uint32_t*>(publish)[threadIdx.x] = __ldcg(reinterpret_cast<const uint32_t*>(w.stats) + threadIdx.x);
-    __threadfence_system();
-  }
+  if (last) publish_stats(w, publish, true);
 }
 
 // One launch runs the pack phases back to back in persistent CTAs (each phase pulls its own
@@ -1495,33 +1494,26 @@ __global__ void __launch_bounds__(256) k_pack_ref(DevState s, BatchIn b, Work w,
   publish_if_last(w, publish);
 }
 
-// pack_variant (pcdn_config) holds launch geometry only: bits 8-11 = CTAs per SM of k_pack (the engine
-// fills in its default, launch_shard_pipeline; 3 if none), bits 12-15 = CTAs per SM of the separate
-// direct pack (default 8 = full occupancy).  Neither changes what is written, only how the persistent
-// CTAs share the work.
-bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
-                 bool has_ref, BatchStats* publish, cudaStream_t st) {
-  // (the CTA counts of pack_variant describe k_pack and k_pack_direct: they do not apply to k_pack_ref)
-  const uint32_t ref_ctas = (uint32_t)n_sms * 8;
+void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_ctas, uint32_t direct_ctas,
+                 int n_sms, bool has_ref, BatchStats* publish, cudaStream_t st) {
+  if (!b.n_bcast && !n_direct) {   // no pack kernel: the counters are final as the control stage left them
+    if (publish) cudaMemcpyAsync(publish, w.stats, sizeof(BatchStats), cudaMemcpyDefault, st);
+    return;
+  }
+  const uint32_t ref_grid = (uint32_t)n_sms * kPackRefCtas;
   if (s.ref_min == 0) {   // shared payload: k_pack_ref is the whole pack
-    if (!b.n_bcast && !n_direct) return false;
-    PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_ctas, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
-    return true;
+    PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_grid, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
+    return;
   }
   // copies; with a message delivered by reference in the batch, k_pack_ref follows on the same stream and is the
   // kernel that publishes the counters
   BatchStats* copy_publish = has_ref ? nullptr : publish;
   const bool direct_separate = n_direct >= kThinSeparateMin;
-  const uint32_t ctas_per_sm = ((pack_variant >> 8) & 15u) ? ((pack_variant >> 8) & 15u) : 3;
-  const uint32_t grid = (uint32_t)n_sms * ctas_per_sm;
   const int do_direct = (n_direct && !direct_separate) ? 1 : 0;
   if (b.n_bcast || do_direct)  // (a batch of nothing but many direct messages has no work for this kernel)
-    PCDN_COUNT_LAUNCH, k_pack<<<grid, 256, 0, st>>>(s, b, w, do_direct, direct_separate ? nullptr : copy_publish);
-  const uint32_t dctas = ((pack_variant >> 12) & 15u) ? ((pack_variant >> 12) & 15u) : 8u;
-  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * dctas, 256, 0, st>>>(s, b, w, copy_publish);
-  const bool launched = direct_separate || b.n_bcast || do_direct;
-  if (has_ref && launched) PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_ctas, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
-  return launched;
+    PCDN_COUNT_LAUNCH, k_pack<<<(uint32_t)n_sms * pack_ctas, 256, 0, st>>>(s, b, w, do_direct, direct_separate ? nullptr : copy_publish);
+  if (direct_separate) PCDN_COUNT_LAUNCH, k_pack_direct<<<(uint32_t)n_sms * direct_ctas, 256, 0, st>>>(s, b, w, copy_publish);
+  if (has_ref) PCDN_COUNT_LAUNCH, k_pack_ref<<<ref_grid, 256, 0, st>>>(s, b, w, n_direct ? 1 : 0, publish);
 }
 
 // =============================================================================== release

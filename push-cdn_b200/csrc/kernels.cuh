@@ -54,6 +54,7 @@ constexpr uint32_t kSmallCtrlConns = 65536;   // largest geometry served by the 
 constexpr uint32_t kSmallCtrlMsgs = 256;      // largest batch it takes
 constexpr uint32_t kSmallCtrlItems = 256;     // ... and at most this many (broadcast, 8192-connection block) match items
 constexpr uint32_t kThinSeparateMin = 2048;  // direct messages in a batch from which the direct pack gets its own launch
+constexpr uint32_t kPackRefCtas = 8;         // CTAs per SM of k_pack_ref (pack_variant does not set them)
 constexpr uint32_t kHotMin = 32;             // more direct hits than this on one connection: ordered by k_dsort_hot
 constexpr uint32_t kHotCtas = 32;            // CTAs (and bitmap scratch rows) of k_dsort_hot
 constexpr uint32_t kCmTileWords = 16;        // bitmap words (512 connections) per cm tile
@@ -244,10 +245,9 @@ struct UpdSlot { uint32_t slot; CuckooEntry e; };
 void launch_apply_updates(const DevState& s, const Upd32* u32, uint32_t n32, const UpdSlot* us,
                           uint32_t nslot, const uint32_t* key_slots, const uint8_t* key_bytes,
                           uint32_t nkeys, cudaStream_t st);
-void launch_batch_begin(const Work& w, cudaStream_t st);
 void launch_parse(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
 void launch_direct(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, cudaStream_t st);
-// zero: the batch's counters, zeroed by k_match / k_ctrl_small before any kernel writes one (null: zeroed earlier)
+// zero: the batch's counters when k_match / k_ctrl_small zeroes them, else null (engine.cu: counters_zeroer)
 // targeted: the batch holds a MSGF_TARGET message (host-staged batches only)
 void launch_match(const DevState& s, const Work& w, const BatchIn& b, BatchStats* zero, bool targeted, cudaStream_t st);
 void launch_plan(const DevState& s, const Work& w, const BatchIn& b, cudaStream_t st);
@@ -258,11 +258,12 @@ void launch_ctrl_small(const DevState& s, const Work& w, const BatchIn& b, bool 
                        BatchStats* publish, bool offsets_only, cudaStream_t st);
 // pool mode: reset what the offsets pass and the pack count before the retry of a refused batch
 void launch_pool_retry_begin(const DevState& s, const Work& w, cudaStream_t st);
-// publish (mapped host memory): the last pack kernel copies the batch's final counters there; returns false when
-// the batch launches no pack kernel, so nothing was published.  has_ref: the batch may hold a message delivered by
-// reference (engines with a threshold launch k_pack_ref after the copy packs; shared-payload engines ignore it)
-bool launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_variant, int n_sms,
-                 bool has_ref, BatchStats* publish, cudaStream_t st);
+// publish (mapped host memory, or null): the last pack kernel copies the batch's final counters there, or a copy on `st`
+// when the batch launches none.  pack_ctas / direct_ctas: CTAs per SM of k_pack / k_pack_direct (they change how the
+// work is shared, not what is written).  has_ref: the batch may hold a message delivered by reference (k_pack_ref
+// follows the copy packs; shared-payload engines ignore it)
+void launch_pack(const DevState& s, const Work& w, const BatchIn& b, uint32_t n_direct, uint32_t pack_ctas, uint32_t direct_ctas,
+                 int n_sms, bool has_ref, BatchStats* publish, cudaStream_t st);
 void launch_release(const DevState& s, const uint32_t* batch_units, const BatchStats* stats, cudaStream_t st);
 void launch_pool_init(const DevState& s, cudaStream_t st);
 unsigned long long kernel_launches();   // launches issued by this library in this process so far

@@ -180,7 +180,7 @@ def test_output_pool_backpressure_and_wrap(pcdn, staged):
 def test_alternating_batch_classes_in_flight(pcdn, pool, pack_variant):
     """The engine moves the pack of short message-major-only batches to its pack stream (so the next
     batch's control kernels run beside it) and decides that from the last COMPLETED batch
-    (engine.cu launch_shard_pipeline).  Several batches are in flight here and their classes alternate
+    (engine.cu batch_begin, batch_pack).  Several batches are in flight here and their classes alternate
     — sparse 4 KiB broadcasts (message-major only), dense 1 KiB broadcasts (connection-major), direct
     only — so successive packs land on different streams in every order; per-connection order and bytes
     must still be the oracle's.  pack_variant 6 << 8: k_pack with 6 CTAs per SM instead of the 3 or 4

@@ -182,7 +182,7 @@ def test_direct_thresholds(pcdn):
 
 
 # ------------------------------------------------------------------ launch geometry
-# pack_variant (kernels.cu launch_pack): bits 8-11 k_pack CTAs per SM, 12-15 k_pack_direct CTAs per SM
+# pack_variant (decoded by pcdn_create): bits 8-11 k_pack CTAs per SM, 12-15 k_pack_direct CTAs per SM
 GEOMETRY = {
     "pack-1cta": 1 << 8, "pack-2cta": 2 << 8, "pack-3cta": 3 << 8, "pack-4cta": 4 << 8, "pack-6cta": 6 << 8,
     "pack-8cta": 8 << 8, "direct-1cta": 1 << 12, "direct-8cta": 8 << 12,
