@@ -5,8 +5,8 @@ import random
 import numpy as np
 import pytest
 
+from gpu_world import World
 from oracle import oracle as orc
-from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
 

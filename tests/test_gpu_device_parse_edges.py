@@ -22,14 +22,12 @@ import numpy as np
 import pytest
 
 import capnp_frames as cf
+from gpu_world import PCDN_ENOSPC, PCDN_EPARSE, PCDN_EPRUNE, World, shard_cfg
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_parity import World, shard_cfg
-from test_gpu_shared_payload import SharedPcdn
 
 pytestmark = pytest.mark.gpu
 
-ENOSPC, EPARSE, EPRUNE = -5, -7, -8
 MAX_KEY = 128                      # pcdn_config_default's max_key_len
 BLOCK = K.kBlockWords * 32        # connections per match block (k_match: one warp per block)
 MAX_CONNS = BLOCK + 256            # two match blocks, the second one eight words long
@@ -48,30 +46,30 @@ def topics_cap(max_batch_msgs):
 
 
 def engine_cfg(pcdn, path, ring=1 << 20):
-    """(package or wrapper, World keyword arguments) of an ingress path"""
+    """World keyword arguments of an ingress path ("shared": the fused path delivering by reference)"""
     base = dict(max_conns=MAX_CONNS, max_keys=16384, ring_bytes_per_conn=ring, batch_slots=16)
     if path == "fused":
-        return pcdn, dict(base, max_batch_msgs=K.kSmallCtrlMsgs, max_batch_bcast=K.kSmallCtrlMsgs)
+        return dict(base, max_batch_msgs=K.kSmallCtrlMsgs, max_batch_bcast=K.kSmallCtrlMsgs)
     if path == "regular":
-        return pcdn, dict(base, max_batch_msgs=1024, max_batch_bcast=1024, flags=pcdn.FLAG_STAGED_SPANS)
+        return dict(base, max_batch_msgs=1024, max_batch_bcast=1024, flags=pcdn.FLAG_STAGED_SPANS)
     if path == "shards":
-        return pcdn, dict(base, max_batch_msgs=1024, max_batch_bcast=1024, **shard_cfg(pcdn, "shards-host"))
-    return SharedPcdn(pcdn), dict(base, max_batch_msgs=K.kSmallCtrlMsgs, max_batch_bcast=K.kSmallCtrlMsgs)
+        return dict(base, max_batch_msgs=1024, max_batch_bcast=1024, **shard_cfg(pcdn, "shards-host"))
+    return dict(base, max_batch_msgs=K.kSmallCtrlMsgs, max_batch_bcast=K.kSmallCtrlMsgs, delivery="shared")
 
 
 def calls_of(pcdn, path):
     """frames per pcdn_receive_frames call: a batch the fused control kernel takes (at most
     kSmallCtrlMsgs messages and kSmallCtrlItems (broadcast, 8192-connection block) items), or more
     than kSmallCtrlMsgs messages for the regular pipeline"""
-    if engine_cfg(pcdn, path)[1]["max_batch_msgs"] <= K.kSmallCtrlMsgs:
+    if engine_cfg(pcdn, path)["max_batch_msgs"] <= K.kSmallCtrlMsgs:
         return min(K.kSmallCtrlMsgs, K.kSmallCtrlItems // -(-MAX_CONNS // (K.kBlockWords * 32)))
     return 3 * K.kSmallCtrlMsgs // 2
 
 
 def make_world(pcdn, path, device_parse, n_valid=N_VALID, ring=1 << 20):
-    pk, kw = engine_cfg(pcdn, path, ring)
+    kw = engine_cfg(pcdn, path, ring)
     kw["flags"] = kw.get("flags", 0) | (pcdn.FLAG_DEVICE_PARSE if device_parse else 0)
-    w = World(pk, n_valid_topics=n_valid, **kw)
+    w = World(pcdn, n_valid_topics=n_valid, **kw)
     rng = random.Random(3)
     keys = [cf.key_of(n) for n in cf.field_sizes(MAX_KEY)[:-1]] + [b"edge-%d" % i for i in range(len(EDGES))]
     conn = 0
@@ -160,12 +158,12 @@ def check(w, frames, device_parse, chunk=200):
     want = []
     for s, o, raw in frames:
         if not device_parse and host_refuses(w, raw, o):
-            want.append(ENOSPC)        # by design: the oracle routes it, the host path refuses it
+            want.append(PCDN_ENOSPC)        # by design: the oracle routes it, the host path refuses it
             continue
         want.append(w.o.broker_receive(raw) if o else w.o.user_receive(s, raw))
     rcs, got, status, n_err, w.batch_msgs = feed(w.pcdn, w.e, frames, chunk)
     if device_parse:
-        bad = [(i, r, x) for i, (r, x) in enumerate(zip(rcs, want)) if r != x and not (r == 0 and x in (EPARSE, EPRUNE))]
+        bad = [(i, r, x) for i, (r, x) in enumerate(zip(rcs, want)) if r != x and not (r == 0 and x in (PCDN_EPARSE, PCDN_EPRUNE))]
         assert not bad, bad[:5]
         deferred = [(i, x) for i, (r, x) in enumerate(zip(rcs, want)) if r == 0 and x < 0]
         first = next((j for j, (s, d) in enumerate(zip(status, deferred)) if s != d[1]), min(len(status), len(deferred)))
@@ -191,7 +189,7 @@ def both_paths(pcdn, path, frames, n_valid=N_VALID, chunk=None):
         rd = check(wd, frames, True, chunk)
         for i, (a, b) in enumerate(zip(rh, rd)):
             refused = host_refuses(wh, frames[i][2], frames[i][1])
-            assert a == b or (b == 0 and a in (EPARSE, EPRUNE)) or (refused and a == ENOSPC and b == 0), (i, a, b)
+            assert a == b or (b == 0 and a in (PCDN_EPARSE, PCDN_EPRUNE)) or (refused and a == PCDN_ENOSPC and b == 0), (i, a, b)
         return rh, rd, (max(wh.batch_msgs, default=0), max(wd.batch_msgs, default=0))
     finally:
         wh.e.close()
@@ -215,7 +213,7 @@ def test_layout_corpus(pcdn, path):
     of the 1024-word first segment, from user and from broker origin"""
     frames = corpus_frames(cf.corpus(MAX_KEY))
     rh, rd, _ = both_paths(pcdn, path, frames)
-    assert rh.count(EPARSE) > 1000 and rd.count(0) > 1500
+    assert rh.count(PCDN_EPARSE) > 1000 and rd.count(0) > 1500
 
 
 # ------------------------------------------------------------------------------------- b. mutation
@@ -275,10 +273,10 @@ def test_topic_lists_in_place(pcdn, path, n_valid):
     path, routed by device parse"""
     frames = topic_frames(n_valid, random.Random(n_valid))
     rh, rd, _ = both_paths(pcdn, path, frames, n_valid)
-    cap = topics_cap(engine_cfg(pcdn, path)[1]["max_batch_msgs"])
+    cap = topics_cap(engine_cfg(pcdn, path)["max_batch_msgs"])
     entries = [len(t) if o else kept(t, n_valid) for t, o in ((orc.deserialize(raw)[1], o) for s, o, raw in frames)]
     refused = [i for i, n in enumerate(entries) if n > cap]
-    assert refused and [i for i, r in enumerate(rh) if r == ENOSPC] == refused
+    assert refused and [i for i, r in enumerate(rh) if r == PCDN_ENOSPC] == refused
     assert all(rd[i] == 0 for i in refused)
 
 
@@ -293,10 +291,10 @@ def test_regular_pipeline_batches_over_one_plan_block(pcdn, path):
              if len(s[1].f1) < 100 and (s[1].kind == cf.DIRECT or len(s[1].f0) <= 9)]
     frames = corpus_frames(specs) + [f for f in topic_frames(N_VALID, rng) if len(orc.deserialize(f[2])[1]) <= 33]
     rng.shuffle(frames)
-    assert len(frames) < engine_cfg(pcdn, path)[1]["max_batch_msgs"]
+    assert len(frames) < engine_cfg(pcdn, path)["max_batch_msgs"]
     rh, rd, largest = both_paths(pcdn, path, frames, chunk=len(frames))
     assert min(largest) > PLAN_CTA_MSGS, largest
-    assert rh.count(EPARSE) > 50 and rd.count(0) > 2 * PLAN_CTA_MSGS
+    assert rh.count(PCDN_EPARSE) > 50 and rd.count(0) > 2 * PLAN_CTA_MSGS
 
 
 # ------------------------------------------------------------------------------------- d. threaded call

@@ -2,48 +2,14 @@
 on the file descriptors must be exactly the byte stream the reference's writer task would put on
 each connection's socket (u32 BE length + raw bytes per message, in order:
 cdn-proto/src/connection/protocols/mod.rs:156-186,354-394), including after soft_close (:287-306)."""
-import ctypes as C
-import os
 import random
-import socket
-import threading
 
 import pytest
 
-from oracle import oracle as orc
-from test_gpu_parity import World, payload, shard_cfg
+import gpu_workloads as workloads
+from gpu_world import World, chunk_streams, shard_cfg, wire
 
 pytestmark = pytest.mark.gpu
-
-
-def wire(frames):
-    """what the writer task sends for these raw frames"""
-    return b"".join(len(f).to_bytes(4, "big") + f for f in frames)
-
-
-def chunk_streams(chunk, out):
-    """walk an EgressChunk record by record (host memory) and append each connection's framed bytes"""
-    for i in range(chunk.n_spans):
-        sp = chunk.spans[i]
-        p = chunk.data + chunk.data_off[i]
-        data = C.string_at(p, sp.len)
-        q = 0
-        for _ in range(sp.n_records):
-            L = int.from_bytes(data[q:q + 4], "big")
-            out.setdefault(sp.conn, bytearray()).extend(data[q:q + 4 + L])
-            q += (4 + L + 31) // 32 * 32
-        assert q == sp.len
-
-
-def traffic(w, rng, keys, n):
-    for _ in range(n):
-        size = rng.choice([0, 5, 100, 1000, 1024, 5000, 20000])
-        if rng.random() < 0.6:
-            t = [rng.randrange(4)]
-            w.bcast(t, orc.broadcast_frame(t, payload(rng, size)))
-        else:
-            k = rng.choice(keys)
-            w.direct(k, orc.direct_frame(k, payload(rng, size)))
 
 
 @pytest.mark.parametrize("mode", ["hbm", "hbm-small-chunks", "host-rings", "shards-host", "pool", "pool-runs-host"])
@@ -66,7 +32,7 @@ def test_drain_to_host_memory_matches_oracle(pcdn, mode):
         w.add_user(k, [x for x in range(4) if rng.random() < 0.4])
     want_total = {}
     for rnd in range(5):   # enough rounds to wrap the rings (two spans per connection)
-        traffic(w, rng, keys, 40)
+        workloads.traffic(w, rng, keys, 40)
         b = w.e.flush()
         got = {}
         st = eg.drain(b, lambda ch: chunk_streams(ch, got))
@@ -85,99 +51,11 @@ def test_drain_to_host_memory_matches_oracle(pcdn, mode):
 def test_writer_to_file_descriptors(pcdn, mode):
     """>= 1 K sinks: every attached connection's memfd must hold exactly the oracle's stream for that
     connection over several batches; connections without a descriptor are counted, not written."""
-    cfg = dict(max_conns=2048, ring_bytes_per_conn=3 << 18)   # 768 KiB: a batch never overflows a ring, several wrap it
-    if mode == "host-rings":
-        cfg["flags"] = pcdn.FLAG_HOST_RINGS
-    if mode == "shards-host":
-        cfg.update(shard_cfg(pcdn, mode), max_conns=1024)
-    if mode == "pool-runs":
-        cfg.update(flags=pcdn.FLAG_OUTPUT_POOL | pcdn.FLAG_SPAN_RUNS, pool_bytes=512 << 20)
-    w = World(pcdn, **cfg)
-    eg = pcdn.Egress(w.e, n_threads=8)
-    rng = random.Random(8)
-    keys = [rng.getrandbits(64).to_bytes(8, "little") * 2 for _ in range(1300)]
-    fds = {}
-    for i, k in enumerate(keys):
-        c = w.add_user(k, [x for x in range(4) if rng.random() < 0.5])
-        if i < 1100:
-            fds[c] = os.memfd_create("conn%d" % c)
-            eg.attach(c, fds[c])
-    stream = {c: bytearray() for c in fds}
-    nbytes = 0
-    for rnd in range(6):
-        traffic(w, rng, keys, 30)
-        b = w.e.flush()
-        st = eg.write_batch(b)
-        assert w.e.poll(b).n_overflow == 0
-        w.e.release_batch(b)
-        exp = w.expect()
-        for c, fr in exp.items():
-            if c in stream:
-                stream[c] += wire(fr)
-        attached_bytes = sum(len(wire(fr)) for c, fr in exp.items() if c in fds)
-        assert st.fd_bytes == attached_bytes
-        assert st.unattached_spans >= sum(1 for c in exp if c not in fds)
-        nbytes += st.fd_bytes
-    assert eg.failed() == []
-    for c, fd in fds.items():
-        os.lseek(fd, 0, os.SEEK_SET)
-        got = os.read(fd, len(stream[c]) + 16)
-        assert got == bytes(stream[c]), c
-        os.close(fd)
-    assert nbytes > 10_000_000
-    eg.close()
-    w.e.close()
+    workloads.writer_to_file_descriptors(pcdn, mode)
 
 
 def test_sockets_backpressure_failure_and_soft_close(pcdn):
     """real sockets: a non-blocking stream socket with a tiny send buffer and a slow reader (partial
     writes, EAGAIN), a peer that went away (write error => reported, like the reference removing the
     user), and soft_close: frames handed to the engine but not even launched yet still go out."""
-    w = World(pcdn, max_conns=256, ring_bytes_per_conn=1 << 20, max_batch_bytes=8 << 20)
-    eg = pcdn.Egress(w.e, n_threads=4)
-    ka, kb, kc = b"alice-key", b"bob-key", b"carol-key"
-    ca, cb_, cc = w.add_user(ka, [0]), w.add_user(kb, [0]), w.add_user(kc, [0])
-    sa, ra = socket.socketpair()
-    sa.setsockopt(socket.SOL_SOCKET, socket.SO_SNDBUF, 4096)
-    sa.setblocking(False)
-    sb, rb = socket.socketpair()
-    rb.close()                      # bob is gone
-    sc, rc_ = socket.socketpair()
-    eg.attach(ca, sa.fileno()); eg.attach(cb_, sb.fileno()); eg.attach(cc, sc.fileno())
-    got_a, got_c = bytearray(), bytearray()
-
-    def reader(sock, buf):
-        while True:
-            d = sock.recv(3000)
-            if not d:
-                return
-            buf.extend(d)
-
-    ta = threading.Thread(target=reader, args=(ra, got_a)); ta.start()
-    tc = threading.Thread(target=reader, args=(rc_, got_c)); tc.start()
-    rng = random.Random(1)
-    for _ in range(30):
-        w.bcast([0], orc.broadcast_frame([0], payload(rng, 30000)))
-    b = w.e.flush()
-    st = eg.write_batch(b)
-    w.e.release_batch(b)
-    assert eg.failed() == [cb_] and eg.failed() == []       # reported once
-    exp = w.expect()
-    want_a, want_c = bytearray(wire(exp[ca])), bytearray(wire(exp[cc]))
-    # the host removes the failed peer, exactly as the reference does
-    w.both("remove_user", kb)
-    # soft_close: these frames are only in the OPEN batch when the close is requested
-    for i in range(5):
-        w.direct(ka, orc.direct_frame(ka, b"last words %d" % i))
-        w.bcast([0], orc.broadcast_frame([0], payload(rng, 2000)))
-    fd = eg.soft_close(ca)
-    assert fd == sa.fileno()
-    exp = w.expect()
-    want_a += wire(exp[ca]); want_c += wire(exp[cc])
-    assert cb_ not in exp
-    sa.close(); sc.close()
-    ta.join(20); tc.join(20)
-    assert bytes(got_a) == bytes(want_a) and bytes(got_c) == bytes(want_c)
-    ra.close(); rc_.close(); sb.close()
-    eg.close()
-    w.e.close()
+    workloads.sockets_backpressure_failure_and_soft_close(pcdn)

@@ -9,112 +9,25 @@ reused while older bytes still wait in a backlog."""
 import fcntl
 import os
 import random
-import socket
 import threading
 import time
 
 import pytest
 
+import gpu_workloads as workloads
+from gpu_world import BIG, PCDN_EINVAL, Reader, backlog_world, flush_until_done, payload, sock_pair, wire
+from gpu_workloads import send_batches
 from oracle import oracle as orc
-from test_gpu_egress import wire
-from test_gpu_parity import World, payload, shard_cfg
-from test_gpu_shared_payload import SharedPcdn
 
 pytestmark = pytest.mark.gpu
 
-MODES = ["rings", "pool", "host-rings", "shards-host", "shared"]
-BIG = 64 << 20
-IDLE_LIMIT = 60.0   # a stalled reader starts by itself after this long, so a writer that waits still ends
-
-
-def make_world(pcdn, mode, **extra):
-    cfg = dict(max_conns=1024, ring_bytes_per_conn=1 << 20, max_batch_bytes=8 << 20, batch_slots=2)
-    p = pcdn
-    if mode == "pool":
-        cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=64 << 20)
-    if mode == "host-rings":
-        cfg.update(flags=pcdn.FLAG_HOST_RINGS)
-    if mode == "shards-host":
-        cfg.update(shard_cfg(pcdn, mode))
-    if mode == "shared":
-        p = SharedPcdn(pcdn)
-    cfg.update(extra)
-    return World(p, **cfg)
-
-
-class Reader:
-    """the receiving end of a socketpair / pipe, read by a thread that starts when go() is called (or
-    by itself after IDLE_LIMIT seconds: then `late` is set and the test fails)"""
-
-    def __init__(self, fd, started=True):
-        self.fd, self.buf, self.late = fd, bytearray(), False
-        self.ev = threading.Event()
-        if started:
-            self.ev.set()
-        self.th = threading.Thread(target=self._run, daemon=True)
-        self.th.start()
-
-    def _run(self):
-        if not self.ev.wait(IDLE_LIMIT):
-            self.late = True
-        while True:
-            try:
-                d = os.read(self.fd, 65536)
-            except OSError:
-                return
-            if not d:
-                return
-            self.buf.extend(d)
-
-    def go(self):
-        self.ev.set()
-
-    def wait_for(self, n, eg=None, timeout=30.0):
-        """the bytes read once n have arrived (eg: moving backlogs on meanwhile, as a host would)"""
-        t = time.time() + timeout
-        while len(self.buf) < n and time.time() < t:
-            if eg is not None:
-                eg.flush_backlog(0)
-            time.sleep(0.005)
-        return bytes(self.buf)
-
-    def finish(self, timeout=30.0):
-        self.th.join(timeout)
-        assert not self.th.is_alive()
-        return bytes(self.buf)
-
-
-def sock_pair(sndbuf=1 << 20):
-    """4096: a stalled peer's buffer; the default asks for 1 MiB (the kernel caps it at its
-    wmem_max, then doubles it), more than one batch's bytes for a peer read by a thread"""
-    s, r = socket.socketpair()
-    s.setsockopt(socket.SOL_SOCKET, socket.SO_SNDBUF, sndbuf)
-    return s, r
-
-
-def send_batches(w, eg, rng, n_batches, topics=(0,), per_batch=8, lo=1, hi=40000, between=None):
-    """n batches of broadcasts of lo..hi bytes, each written then released at once; returns the
-    oracle's stream per connection"""
-    want = {}
-    for k in range(n_batches):
-        for _ in range(per_batch):
-            t = [rng.choice(topics)]
-            w.bcast(t, orc.broadcast_frame(t, payload(rng, rng.randint(lo, hi))))
-        b = w.e.flush()
-        eg.write_batch(b)
-        w.e.release_batch(b)
-        for c, fr in w.expect().items():
-            want.setdefault(c, bytearray()).extend(wire(fr))
-        if between:
-            between(k, want)
-    return want
-
-
-def flush_until_done(eg, timeout=30.0):
-    t = time.time() + timeout
-    while eg.flush_backlog(100) and time.time() < t:
-        pass
-    return eg.flush_backlog(0)
+# (layout, delivery) under this file's test ids
+RINGS = pytest.param("rings", "copy", id="rings")
+POOL = pytest.param("pool", "copy", id="pool")
+HOST = pytest.param("host", "copy", id="host-rings")
+SHARDS = pytest.param("shards-host", "copy", id="shards-host")
+SHARED = pytest.param("rings", "shared", id="shared")
+MODES = [RINGS, POOL, HOST, SHARDS, SHARED]
 
 
 def shard_of(w, c):
@@ -126,52 +39,20 @@ def shard_of(w, c):
 
 
 # ------------------------------------------------------------------ a stalled peer
-@pytest.mark.parametrize("mode", MODES)
-def test_stalled_peer_does_not_stall_the_others(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", MODES)
+def test_stalled_peer_does_not_stall_the_others(pcdn, name, delivery):
     """A (4 KiB send buffer, blocking socket) reads nothing; B and C are read by threads.  Six batches
     of 1 B - 40 KB broadcasts are written and released at once: every call returns, B and C hold
     their whole streams, A is not failed.  Then A's reader runs and flush_backlog completes A."""
-    w = make_world(pcdn, mode)
-    eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=BIG, backlog_bytes_total=4 * BIG)
-    rng = random.Random(11)
-    conns = [w.add_user(b"user-%03d" % i, [0]) for i in range(12)]   # three shards: spread A, B, C
-    a, b, c = conns[0], conns[4], conns[8]
-    sa, ra = sock_pair(4096)
-    sb, rb = sock_pair()
-    sc, rc_ = sock_pair()
-    eg.attach(a, sa.fileno()); eg.attach(b, sb.fileno()); eg.attach(c, sc.fileno())
-    reader_a = Reader(ra.fileno(), started=False)
-    reader_b, reader_c = Reader(rb.fileno()), Reader(rc_.fileno())
-    t0 = time.time()
-    want = send_batches(w, eg, rng, 6)
-    assert time.time() - t0 < IDLE_LIMIT / 2 and not reader_a.late
-    assert reader_b.wait_for(len(want[b]), eg) == bytes(want[b])
-    assert reader_c.wait_for(len(want[c]), eg) == bytes(want[c])
-    assert eg.failed() == []
-    pend, nbytes = eg.backlog()
-    assert pend == [a] and 0 < nbytes < len(want[a])
-    assert len(reader_a.buf) == 0
-    reader_a.go()
-    assert flush_until_done(eg) == 0
-    assert eg.backlog() == ([], 0)
-    assert reader_a.wait_for(len(want[a])) == bytes(want[a])
-    assert eg.failed() == []
-    for s in (sa, sb, sc):
-        s.close()
-    for r in (reader_a, reader_b, reader_c):
-        r.finish()
-    for s in (ra, rb, rc_):
-        s.close()
-    eg.close()
-    w.e.close()
+    workloads.stalled_peer_does_not_stall_the_others(pcdn, name, delivery)
 
 
 # ------------------------------------------------------------------ budgets
-@pytest.mark.parametrize("mode", ["rings", "pool", "shared"])
-def test_per_connection_budget(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, POOL, SHARED])
+def test_per_connection_budget(pcdn, name, delivery):
     """A's backlog would outgrow backlog_bytes_per_conn: A is reported exactly once and detached, it
     received a prefix of its stream, B and C are complete, the backlog total returns to 0"""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=96 << 10)
     rng = random.Random(12)
     a, b, c = (w.add_user(k, [0]) for k in (b"alice", b"bob", b"carol"))
@@ -204,18 +85,18 @@ def test_per_connection_budget(pcdn, mode):
     w.e.close()
 
 
-@pytest.mark.parametrize("mode", ["rings", "shards-host"])
-def test_total_budget_two_stalled_peers(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, SHARDS])
+def test_total_budget_two_stalled_peers(pcdn, name, delivery):
     """two stalled peers (on different shards with three shards) under backlog_bytes_total: first both
     backlog ~100 KB, then ~100 KB more for A1 alone — A1's own backlog stays under the budget, the two
     together cross it.  A1 is reported; A2 still receives its whole stream."""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     budget = 260 << 10
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_total=budget)
     rng = random.Random(13)
     users = [w.add_user(b"user-%03d" % i, []) for i in range(12)]
     a1 = users[0]
-    a2 = next(u for u in users[1:] if shard_of(w, u) != shard_of(w, a1)) if mode == "shards-host" else users[1]
+    a2 = next(u for u in users[1:] if shard_of(w, u) != shard_of(w, a1)) if name == "shards-host" else users[1]
     w.both("subscribe_user_to", b"user-%03d" % users.index(a1), [0, 1])
     w.both("subscribe_user_to", b"user-%03d" % users.index(a2), [0])
     s1, r1 = sock_pair(4096)
@@ -253,11 +134,11 @@ def test_total_budget_two_stalled_peers(pcdn, mode):
 
 
 # ------------------------------------------------------------------ order
-@pytest.mark.parametrize("mode", MODES)
-def test_partly_drained_backlog_keeps_fifo(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", MODES)
+def test_partly_drained_backlog_keeps_fifo(pcdn, name, delivery):
     """between batches the peer reads a little and flush_backlog(0) moves part of the backlog on; the
     next batch's records must still go behind what is left: one FIFO stream per connection"""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=BIG)
     rng = random.Random(14)
     conns = [w.add_user(b"user-%03d" % i, [0]) for i in range(6)]
@@ -302,11 +183,11 @@ def test_partly_drained_backlog_keeps_fifo(pcdn, mode):
 
 
 # ------------------------------------------------------------------ lifecycle
-@pytest.mark.parametrize("mode", ["rings", "pool", "shared"])
-def test_soft_close_writes_the_backlog(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, POOL, SHARED])
+def test_soft_close_writes_the_backlog(pcdn, name, delivery):
     """a backlogged connection is soft-closed with its reader running: soft_close returns the fd once
     the whole stream (the backlog, then frames of the batch still open at the close) is written"""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=BIG)
     rng = random.Random(15)
     ka = b"alice"
@@ -335,12 +216,12 @@ def test_soft_close_writes_the_backlog(pcdn, mode):
     w.e.close()
 
 
-@pytest.mark.parametrize("mode", ["rings", "shards-host"])
-def test_detach_drops_the_backlog_and_a_reused_id_starts_clean(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, SHARDS])
+def test_detach_drops_the_backlog_and_a_reused_id_starts_clean(pcdn, name, delivery):
     """detach drops the connection's backlog at once (the total returns to 0, nothing is written to
     it later); after the id's quarantine a new user gets the same id on a new socket and receives
     only its own records"""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=BIG)
     rng = random.Random(16)
     ka = b"alice"
@@ -385,11 +266,11 @@ def test_detach_drops_the_backlog_and_a_reused_id_starts_clean(pcdn, mode):
 
 
 # ------------------------------------------------------------------ other descriptors
-@pytest.mark.parametrize("mode", ["rings", "shared"])
-def test_non_blocking_pipe_takes_the_writev_path(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, SHARED])
+def test_non_blocking_pipe_takes_the_writev_path(pcdn, name, delivery):
     """a pipe is not a socket: the writer uses writev, and a non-blocking pipe of 4096 bytes answers
     EAGAIN; its backlog drains once the pipe is read"""
-    w = make_world(pcdn, mode)
+    w = backlog_world(pcdn, name, delivery)
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=BIG)
     rng = random.Random(17)
     a, b = w.add_user(b"alice", [0]), w.add_user(b"bob", [0])
@@ -416,11 +297,11 @@ def test_non_blocking_pipe_takes_the_writev_path(pcdn, mode):
     w.e.close()
 
 
-@pytest.mark.parametrize("mode", ["rings", "shards-host", "shared"])
-def test_memfds_same_bytes_and_writes_with_and_without_backlog(pcdn, mode):
+@pytest.mark.parametrize("name,delivery", [RINGS, SHARDS, SHARED])
+def test_memfds_same_bytes_and_writes_with_and_without_backlog(pcdn, name, delivery):
     """a descriptor that always takes everything never backlogs: each batch written by an egress with
     a backlog and by one without gives the same fd_bytes, fd_writes and records, and the same files"""
-    w = make_world(pcdn, mode, batch_slots=4)
+    w = backlog_world(pcdn, name, delivery, batch_slots=4)
     plain = pcdn.Egress(w.e, n_threads=4)
     backlogged = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=1 << 20, backlog_bytes_total=1 << 20)
     rng = random.Random(18)
@@ -458,7 +339,7 @@ def test_old_config_size_means_no_backlog(pcdn):
     it always did: it waits for the slow reader (nothing is backlogged even though the fields behind
     the old size are set), so write_batch returns with every byte in the socket; any other size is
     refused"""
-    w = make_world(pcdn, "rings")
+    w = backlog_world(pcdn, "rings")
     eg = pcdn.Egress(w.e, n_threads=4, backlog_bytes_per_conn=1, backlog_bytes_total=1,
                      struct_size=pcdn.EGRESS_CONFIG_NO_BACKLOG_SIZE)
     rng = random.Random(19)
@@ -487,5 +368,5 @@ def test_old_config_size_means_no_backlog(pcdn):
     eg.close()
     with pytest.raises(pcdn.PcdnError) as ei:
         pcdn.Egress(w.e, struct_size=pcdn.EGRESS_CONFIG_NO_BACKLOG_SIZE + 8)
-    assert ei.value.code == -1            # PCDN_EINVAL
+    assert ei.value.code == PCDN_EINVAL
     w.e.close()

@@ -6,8 +6,8 @@ import random
 
 import pytest
 
+from gpu_world import World, payload, shard_cfg
 from oracle import oracle as orc
-from test_gpu_parity import World, payload, shard_cfg
 
 pytestmark = pytest.mark.gpu
 

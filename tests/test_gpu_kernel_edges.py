@@ -4,100 +4,16 @@ against the oracle, or against an exact numpy model where the oracle would be to
 
 Every threshold comes from kernels.cuh through kconst.K, so the cases stay on both sides of a limit
 when it is retuned."""
-import ctypes
 import random
 
 import numpy as np
 import pytest
 
+from gpu_world import EDGE_SLOTS, World, check, edge_sizes, edge_world, raw, records, span_table, units
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
-
-TILE_BYTES = K.kFatTileBytes   # bytes of stores a message-major tile aims at
-
-
-def vec_bytes(raw_len):
-    return (4 + raw_len + 15) // 16 * 16
-
-
-def units(raw_len):
-    return (4 + raw_len + K.kUnit - 1) // K.kUnit
-
-
-def tile_recipients(raw_len):
-    return max(32, min(K.kTileRecipients, TILE_BYTES // min(vec_bytes(raw_len), K.kChunkBytes)))
-
-
-def raw(n, tag):
-    """n bytes that differ from vector to vector and from message to message"""
-    return ((np.arange(n, dtype=np.int64) * 7 + tag * 13) % 251).astype(np.uint8).tobytes()
-
-
-def edge_sizes():
-    """raw lengths around every size threshold of the pack: b - 4, b - 1, b, b + 1, b + 4 (the 4-byte length
-    prefix moves the 16-byte vector and 32-byte unit steps)"""
-    out = set()
-    for b in (K.kCmMaxBytes - 4,                   # largest record on the connection-major path
-              K.kChunkBytes - 4,                   # one staging chunk
-              2 * K.kChunkBytes - 4):              # two chunks
-        out.update((b - 4, b - 1, b, b + 1, b + 4))
-    return sorted(out)
-
-
-# ------------------------------------------------------------------ a world whose every slot is a user
-EDGE_SLOTS = 2 * 32 * K.kBlockWords   # two match blocks
-
-
-def edge_conns(n):
-    """k_offsets CTA (256), connection-major tile (32 * kCmTileWords), match block (32 * kBlockWords) edges"""
-    tile, blk = 32 * K.kCmTileWords, 32 * K.kBlockWords
-    return sorted({0, 255, 256, 257, tile - 1, tile, tile + 1, blk - 1, blk, blk + 1, n - 1})
-
-
-def recipient_counts(n):
-    dense = n >> K.kCmDenseShift
-    out = {K.kFatMin - 1, K.kFatMin, K.kFatMin + 1, dense - 1, dense, dense + 1}
-    for s in edge_sizes():
-        out.update((tile_recipients(s), tile_recipients(s) + 1))
-    return sorted(out)
-
-
-def edge_world(pcdn, **cfg):
-    """World with EDGE_SLOTS users (connection c = user c); topic i reaches exactly recipient_counts()[i]
-    users, every edge connection among them.  → (world, keys, {recipient count: topic})"""
-    kw = dict(max_conns=EDGE_SLOTS, max_keys=EDGE_SLOTS + 1024, ring_bytes_per_conn=1 << 19)
-    kw.update(cfg)
-    w = World(pcdn, **kw)
-    n = w.e.shard_info(0).shard_stride
-    assert n == EDGE_SLOTS
-    rng = random.Random(1)
-    edges = edge_conns(n)
-    others = sorted(set(range(n)) - set(edges))
-    subs = [[] for _ in range(n)]
-    counts = recipient_counts(n)
-    for t, d in enumerate(counts):
-        for c in edges + rng.sample(others, d - len(edges)):
-            subs[c].append(t)
-    keys = [c.to_bytes(4, "little") + b"edge" for c in range(n)]
-    kb = np.frombuffer(b"".join(keys), dtype=np.uint8).reshape(n, 8)
-    offs = np.concatenate([[0], np.cumsum([len(s) for s in subs])]).astype(np.uint32)
-    tp = np.array([t for s in subs for t in s], dtype=np.uint16)
-    assert np.array_equal(w.e.add_users_bulk(kb, 8, tp, offs), np.arange(n))
-    for c in range(n):
-        w.map[c] = w.o.add_user(keys[c], subs[c])
-    return w, keys, {d: t for t, d in enumerate(counts)}
-
-
-def check(w):
-    """w.check(), after which the oracle forgets the frames it compared (it would copy its whole streams again
-    at every later check)"""
-    n = w.check()
-    w.o.clear()
-    w.taken.clear()
-    return n
 
 
 PACK_MODES = [(out, ctrl) for out in ("rings", "pool") for ctrl in ("fused", "regular")]
@@ -232,24 +148,6 @@ def test_cta_count_invariance(pcdn, out):
 FULL_SLOTS = (1 << 20) + 65536   # 136 x 8192: the k_pool_finish grid is min(SMs, slots / 8192) = every SM
 
 
-def span_table(res):
-    """every span of a batch as int64 rows (conn, ring_off, len, n_records) sorted by connection and offset;
-    the run-length form expanded (entry k of a run: conn0 + k at ring_off + k * off_stride)"""
-    if res.n_spans == 0:
-        return np.zeros((0, 4), dtype=np.int64)
-    u32 = ctypes.POINTER(ctypes.c_uint32)
-    if res.runs:
-        r = np.ctypeslib.as_array(ctypes.cast(res.runs, u32), shape=(res.n_runs, 6)).astype(np.int64)
-        n = r[:, 1]
-        k = np.arange(int(n.sum())) - np.repeat(np.cumsum(n) - n, n)
-        t = np.stack([np.repeat(r[:, 0], n) + k, np.repeat(r[:, 2], n) + k * np.repeat(r[:, 5], n),
-                      np.repeat(r[:, 3], n), np.repeat(r[:, 4], n)], axis=1)
-    else:
-        t = np.ctypeslib.as_array(ctypes.cast(res.spans, u32), shape=(res.n_spans, 4)).astype(np.int64)
-    assert len(t) == res.n_spans
-    return t[np.lexsort((t[:, 1], t[:, 0]))]
-
-
 def read_frames(e, res, t, conn, pool):
     """the frames a socket writer would send for `conn` (pcdn_read of its spans; a wrapped ring's piece
     that does not start at offset 0 comes first)"""
@@ -257,13 +155,7 @@ def read_frames(e, res, t, conn, pool):
     pieces = sorted(t[lo:hi, 1:].tolist(), key=lambda p: (p[0] == 0 and hi - lo > 1, p[0]))
     out = []
     for off, ln, nrec in pieces:
-        data = e.read(conn, res.pool_base + off if pool else off, ln)
-        p = 0
-        for _ in range(nrec):
-            n = int.from_bytes(data[p:p + 4], "big")
-            out.append(data[p + 4:p + 4 + n])
-            p += units(n) * K.kUnit
-        assert p == ln
+        out += records(e.read(conn, res.pool_base + off if pool else off, ln), nrec)
     return out
 
 

@@ -15,14 +15,13 @@ import random
 
 import pytest
 
+from gpu_world import PCDN_ENOSPC, World
 import keyhash as kh
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
 
-ENOSPC = -5
 SEEDS = [0, 0xF00DFACE12345679]          # 0: the built-in seed
 SEED_IDS = ["builtin-seed", "top-bit-seed"]
 MAX_KEYS = 256                           # 128 buckets
@@ -73,7 +72,7 @@ class Lookup:
         self.touched.add(key)
         with pytest.raises(self.pcdn.PcdnError) as ei:
             self.w.e.add_user(key, [])
-        assert ei.value.code == ENOSPC
+        assert ei.value.code == PCDN_ENOSPC
 
     def remove(self, key):
         self.touched.add(key)

@@ -17,43 +17,48 @@ n_overflow, n_direct_dropped and status must be what the oracle delivered for it
 the oracle's."""
 import pytest
 
+from gpu_world import STATUS_EAGAIN, Sends, World, layout, user_sync
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_pool_retry import EAGAIN
-from test_gpu_send_to_brokers import Sends, user_sync
-from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
 
 N_USERS = 600
 T_REF = 4096   # ref_min_bytes of the threshold classes
 
-# kernel launches of one batch of each class (the retry classes: its first launch, then the retry)
+# per class: the kernel launches of one batch (the retry classes: its first launch, then the retry), and the
+# engine's layout and delivery
 LAUNCHES = {
-    "fused-broadcast": 2,
-    "fused-direct": 2,
-    "regular-broadcast-one-block": 4,
-    "regular-broadcast-blocks": 6,
-    "device-parse-fused": 3,
-    "device-parse-regular": 5,
-    "direct-only": 6,
-    "pool-fused": 2,
-    "pool-regular": 5,
-    "pool-retry-fused": (2, 3),
-    "pool-retry-regular": (8, 4),
-    "ref-below-threshold": 2,
-    "ref-at-threshold": 3,
-    "shared-payload": 2,
-    "targeted-fused": 2,
-    "targeted-regular": 4,
+    "fused-broadcast": (2, "rings", "copy"),
+    "fused-direct": (2, "rings", "copy"),
+    "regular-broadcast-one-block": (4, "staged", "copy"),
+    "regular-broadcast-blocks": (6, "staged", "copy"),
+    "device-parse-fused": (3, "devparse", "copy"),
+    "device-parse-regular": (5, "devparse-staged", "copy"),
+    "direct-only": (6, "rings", "copy"),
+    "pool-fused": (2, "pool", "copy"),
+    "pool-regular": (5, "pool-staged", "copy"),
+    "pool-retry-fused": ((2, 3), "pool", "copy"),
+    "pool-retry-regular": ((8, 4), "pool-staged", "copy"),
+    "ref-below-threshold": (2, "rings", ("ref", T_REF)),
+    "ref-at-threshold": (3, "rings", ("ref", T_REF)),
+    "shared-payload": (2, "rings", "shared"),
+    "targeted-fused": (2, "rings", "copy"),
+    "targeted-regular": (4, "staged", "copy"),
 }
 
 
 class Seq(Sends, World):
     """users on topics 0 / 1 and one peer broker on topic 0; a warm-up batch takes the table changes to the device"""
 
-    def __init__(self, pcdn, **cfg):
-        super().__init__(pcdn, max_conns=1024, **cfg)
+    def __init__(self, pcdn, case):
+        _, name, delivery = LAUNCHES[case]
+        cfg = layout(pcdn, name)
+        if case.startswith("pool-retry"):
+            cfg.update(pool_bytes=4 << 20, batch_slots=4)
+        elif name.startswith("pool"):
+            cfg["pool_bytes"] = 64 << 20
+        super().__init__(pcdn, max_conns=1024, delivery=delivery, **cfg)
         self.keys = [b"user-%04d" % i for i in range(N_USERS)]
         for i, k in enumerate(self.keys):
             self.add_user(k, [i % 2])
@@ -100,24 +105,9 @@ def directs(w, n, size=200):
         w.direct(k, frame(j, size))
 
 
-def engine_cfg(pcdn, case):
-    staged = pcdn.FLAG_STAGED_SPANS if "regular" in case else 0
-    if case.startswith("device-parse"):
-        return dict(flags=pcdn.FLAG_DEVICE_PARSE | staged)
-    if case.startswith("pool-retry"):
-        return dict(flags=pcdn.FLAG_OUTPUT_POOL | staged, pool_bytes=4 << 20, batch_slots=4)
-    if case.startswith("pool"):
-        return dict(flags=pcdn.FLAG_OUTPUT_POOL | staged, pool_bytes=64 << 20)
-    if case.startswith("ref"):
-        return dict(ref_min_bytes=T_REF)
-    if case == "shared-payload":
-        return dict(flags=pcdn.FLAG_SHARED_PAYLOAD)
-    return dict(flags=staged)
-
-
 @pytest.mark.parametrize("case", [c for c in LAUNCHES if not c.startswith("pool-retry")])
 def test_launches_and_counters(pcdn, case):
-    w = Seq(pcdn, **engine_cfg(pcdn, case))
+    w = Seq(pcdn, case)
     drops = 0
     if case == "regular-broadcast-blocks":
         broadcasts(w, 300, 100)                      # 300 messages: three plan passes
@@ -141,7 +131,7 @@ def test_launches_and_counters(pcdn, case):
             w.bcast([1], frame(1, T_REF - 1))
         if case == "ref-at-threshold":
             w.bcast([1], frame(1, T_REF))
-    assert w.batch(drops) == LAUNCHES[case], case
+    assert w.batch(drops) == LAUNCHES[case][0], case
     w.e.close()
 
 
@@ -150,7 +140,7 @@ def test_pool_retry_launches_and_counters(pcdn, control):
     """a batch the output pool refuses launches its class's kernels; its retry launches k_pool_retry_begin and the
     passes that place and pack it, and then carries the counters of what it delivers"""
     case = "pool-retry-" + control
-    w = Seq(pcdn, **engine_cfg(pcdn, case))
+    w = Seq(pcdn, case)
     hot = w.keys[0]
     for j in range(38):                              # 3.8 MB of the 4 MiB pool, unreleased
         w.direct(hot, frame(j, 100_000))
@@ -158,12 +148,12 @@ def test_pool_retry_launches_and_counters(pcdn, control):
     broadcasts(w, 12)                                # 1.2 MB: fits the pool, not beside the first batch
     directs(w, 3)
     n1, b1, r1, want1 = w.launch()
-    assert r1.status == EAGAIN
+    assert r1.status == STATUS_EAGAIN
     w.finish(b0, r0, want0)
     n0 = w.e.stats().kernel_launches
     w.e.retry_batch(b1)
     r1 = w.e.poll(b1)
     n_retry = w.e.stats().kernel_launches - n0
     w.finish(b1, r1, want1)
-    assert (n1, n_retry) == LAUNCHES[case]
+    assert (n1, n_retry) == LAUNCHES[case][0]
     w.e.close()

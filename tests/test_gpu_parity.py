@@ -8,7 +8,9 @@ import numpy as np
 
 import pytest
 
+import gpu_workloads as workloads
 import scenarios
+from gpu_world import PCDN_EAGAIN, World, payload
 from harness import EngineBackend
 from oracle import oracle as orc
 
@@ -28,136 +30,7 @@ def test_reference_scenario_host_rings(pcdn, scenario):
     scenario(EngineBackend(pcdn, flags=pcdn.FLAG_HOST_RINGS))
 
 
-# ------------------------------------------------------------------ differential harness
-class World:
-    """drives engine and oracle with identical calls and compares delivered frames
-    (record=True: also keeps the engine calls and the oracle's frames of every check(), so that
-    replay() can run the same workload on engines of other configurations against this ONE oracle run)"""
-
-    def __init__(self, pcdn, n_valid_topics=0, record=False, **cfg):
-        kw = dict(max_conns=8192, max_topics=256, max_keys=16384, ring_bytes_per_conn=1 << 18,
-                  max_batch_msgs=4096, max_batch_bcast=512, max_batch_bytes=32 << 20,
-                  max_batch_deliveries=1 << 20, identity="/", n_valid_topics=n_valid_topics)
-        kw.update(cfg)
-        self.pcdn = pcdn
-        self.cfg = kw
-        self.e = pcdn.Engine(**kw)
-        self.o = orc.Oracle("/", n_valid_topics)
-        self.map = {}
-        self.taken = {}
-        self.calls = [] if record else None
-
-    def _engine(self, name, *a):
-        r = getattr(self.e, name)(*a)
-        if self.calls is not None:
-            self.calls.append((name, a, r))
-        return r
-
-    def add_user(self, key, topics):
-        c = self._engine("add_user", key, topics)
-        self.map[c] = self.o.add_user(key, topics)
-        return c
-
-    def add_broker(self, ident, topics=()):
-        c = self._engine("add_broker", ident)
-        self.map[c] = self.o.add_broker(ident)
-        if topics:
-            self.both("subscribe_broker_to", ident, list(topics))
-        return c
-
-    def both(self, name, *a):
-        self._engine(name, *a)
-        getattr(self.o, name)(*a)
-
-    def bcast(self, topics, raw, to_users_only=False):
-        self.both("handle_broadcast_message", topics, raw, to_users_only)
-
-    def direct(self, rcpt, raw, to_user_only=False):
-        self.both("handle_direct_message", rcpt, raw, to_user_only)
-
-    def expect(self):
-        """oracle frames per ENGINE conn id since the last call"""
-        out = {}
-        for ec, oc in self.map.items():
-            fr = self.o.frames(oc)
-            k = self.taken.get(oc, 0)
-            if len(fr) > k:
-                out[ec] = fr[k:]
-            self.taken[oc] = len(fr)
-        return out
-
-    def check(self):
-        got = self.e.drain()
-        want = self.expect()
-        if self.calls is not None:
-            self.calls.append(("check", (), want))
-        return self.compare(self.e, got, want)
-
-    def replay(self, **cfg):
-        """the recorded engine calls on a fresh engine configured like this one updated by `cfg`; every
-        batch must deliver the oracle frames recorded for it"""
-        e = self.pcdn.Engine(**{**self.cfg, **cfg})
-        try:
-            for name, a, r in self.calls:
-                if name == "check":
-                    self.compare(e, e.drain(), r)
-                else:
-                    assert getattr(e, name)(*a) == r, name
-        finally:
-            e.close()
-
-    def compare(self, e, got, want):
-        bad = [c for c in sorted(set(got) | set(want)) if got.get(c, []) != want.get(c, [])]
-        if bad:
-            self.dump(e, bad, got, want)
-        assert set(got) == set(want), (sorted(set(got) ^ set(want))[:10])
-        for c in want:
-            assert len(got[c]) == len(want[c]), (c, len(got[c]), len(want[c]))
-            for i, (g, w) in enumerate(zip(got[c], want[c])):
-                assert g == w, f"conn {c} frame {i}: {len(g)} vs {len(w)} bytes"
-        return sum(len(v) for v in want.values())
-
-    def dump(self, e, bad, got, want):
-        """diagnostics for a failing comparison (pytest shows them with the failure)"""
-        import sys
-        f = sys.stdout
-        f.write(f"==== {len(bad)} bad connections of {len(want)}; first: {bad[:20]}\n")
-        r = e.last_result
-        f.write(f"last batch: msgs={r.n_msgs} deliveries={r.n_deliveries} spans={r.n_spans} overflow={r.n_overflow} "
-                f"dropped={r.n_direct_dropped} status={r.status}\n")
-        for c in bad[:6]:
-            g, w = got.get(c, []), want.get(c, [])
-            f.write(f"conn {c}: got {len(g)} frames, want {len(w)}\n")
-            sig = lambda fr: (len(fr), fr[:4].hex(), fr[-12:].hex())
-            f.write("  got : " + " ".join(str(sig(x)) for x in g[:40]) + "\n")
-            f.write("  want: " + " ".join(str(sig(x)) for x in w[:40]) + "\n")
-            for i, (a, b) in enumerate(zip(g, w)):
-                if a != b and len(a) == len(b):
-                    d = next(k for k in range(len(a)) if a[k] != b[k])
-                    f.write(f"  frame {i}: same length {len(a)}, first diff at byte {d}: {a[d:d+16].hex()} vs {b[d:d+16].hex()}\n")
-                    break
-
-
-def payload(rng, n):
-    return bytes(rng.getrandbits(8) for _ in range(min(n, 64))) * (n // 64 + 1)
-
-
-def shard_cfg(pcdn, variant):
-    """engine config of the sharded variants: 'shards-host' = three connection shards that share GPU 0
-    (every shard copies the batch from pinned host memory: runs on a one-GPU box); 'shards-nccl' = one
-    shard per GPU, the library moves every batch with ncclBroadcast (needs >= 2 GPUs)"""
-    import torch
-
-    if variant == "shards-host":
-        return dict(devices=[0, 0, 0], ingest=pcdn.INGEST_HOST)
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    return dict(devices=list(range(min(n, 4))), ingest=pcdn.INGEST_NCCL)
-
-
-@pytest.mark.parametrize("variant", [0, "staged", "runs", "runs-staged", "pool", "pool-staged-runs", "pool-host", "pool-shards", "pool-shards-nccl",
-                                     "pool-shards-staged", "host", "shards-host", "shards-host-staged", "shards-nccl"])
+@pytest.mark.parametrize("variant", workloads.MIXED_LAYOUTS)
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_random_mixed_batches(pcdn, seed, variant):
     """users + peer brokers, multi-topic broadcasts (fat and thin recipient sets), directs to local,
@@ -167,73 +40,7 @@ def test_random_mixed_batches(pcdn, seed, variant):
     The 'shards-*' variants run the SAME workload on ONE engine whose connections are spread over
     several shards (pcdn_config.devices) and compare with the same single unsharded oracle; the
     '*-staged' ones force the regular control kernels there, so they run with conn_base != 0."""
-    rng = random.Random(seed)
-    if variant == "staged":
-        w = World(pcdn, flags=pcdn.FLAG_STAGED_SPANS, ring_bytes_per_conn=1 << 20)
-    elif variant.startswith("pool") if isinstance(variant, str) else False:
-        # PCDN_FLAG_OUTPUT_POOL: one shared output pool (1 GiB; a batch here delivers a few hundred MB)
-        # instead of per-connection rings
-        fl = pcdn.FLAG_OUTPUT_POOL
-        kw = {}
-        if variant == "pool-staged-runs":
-            fl |= pcdn.FLAG_STAGED_SPANS | pcdn.FLAG_SPAN_RUNS
-        if variant == "pool-host":
-            fl |= pcdn.FLAG_HOST_RINGS
-        if variant in ("pool-shards", "pool-shards-staged"):
-            kw.update(shard_cfg(pcdn, "shards-host"), max_conns=1024)
-        if variant == "pool-shards-staged":
-            fl |= pcdn.FLAG_STAGED_SPANS
-        if variant == "pool-shards-nccl":   # every GPU its own pool, batches replicated by the library's ncclBroadcast
-            kw.update(shard_cfg(pcdn, "shards-nccl"), max_conns=1024)
-            fl |= pcdn.FLAG_SPAN_RUNS
-        w = World(pcdn, flags=fl, pool_bytes=1 << 30, **kw)
-    elif variant in ("runs", "runs-staged"):
-        # run-length span table (PCDN_FLAG_SPAN_RUNS): same streams, the table just arrives compressed
-        w = World(pcdn, flags=pcdn.FLAG_SPAN_RUNS | (pcdn.FLAG_STAGED_SPANS if variant == "runs-staged" else 0), ring_bytes_per_conn=1 << 20)
-    elif variant == "host":
-        # egress hand-off mode: rings in mapped pinned host memory, frames read in place by the host
-        # (TMA bulk stores over PCIe)
-        w = World(pcdn, flags=pcdn.FLAG_HOST_RINGS, ring_bytes_per_conn=1 << 20, max_conns=2048)
-        assert w.e.host_rings() != 0
-    elif isinstance(variant, str):
-        staged = variant.endswith("-staged")
-        w = World(pcdn, ring_bytes_per_conn=1 << 20, max_conns=1024, flags=pcdn.FLAG_STAGED_SPANS if staged else 0,
-                  **shard_cfg(pcdn, variant.removesuffix("-staged")))
-        assert w.e.num_shards()[0] >= 2
-    else:
-        w = World(pcdn, ring_bytes_per_conn=1 << 20)
-    keys = []
-    for i in range(1500):
-        k = rng.getrandbits(64).to_bytes(8, "little") * rng.choice([1, 4, 16])
-        keys.append(k)
-        # topic 0 is popular (fat path), topics 10+ are rare (thin path)
-        t = [x for x in range(16) if rng.random() < (0.6 if x == 0 else 0.1 if x < 10 else 0.004)]
-        w.add_user(k, t)
-    for b in range(3):
-        w.add_broker(f"b{b}/p{b}", [rng.randrange(16) for _ in range(3)])
-    remote = [b"remote%d" % i for i in range(8)]
-    w.both("apply_user_sync", "b1/p1", [(k, 1, "b1/p1") for k in remote])
-    total = 0
-    for batch in range(4):
-        for j in range(rng.randrange(20, 120)):
-            r = rng.random()
-            size = rng.choice([0, 1, 11, 12, 13, 100, 1024, 4096, 16000, 16384, 20000, 40000]) if rng.random() < 0.5 \
-                else rng.randrange(0, 3000)
-            if r < 0.55:
-                topics = [rng.randrange(16) for _ in range(rng.randrange(1, 4))]
-                if rng.random() < 0.4:
-                    topics.append(0)
-                w.bcast(topics, orc.broadcast_frame([t for t in topics], payload(rng, size)), rng.random() < 0.3)
-            else:
-                rc = rng.choice(keys) if rng.random() < 0.7 else rng.choice(remote + [b"nobody", b""])
-                w.direct(rc, orc.direct_frame(rc, payload(rng, size)), rng.random() < 0.3)
-        if batch == 2:  # state change between batches
-            for k in rng.sample(keys, 50):
-                w.both("remove_user", k)
-            for k in rng.sample(keys, 50):
-                w.both("subscribe_user_to", k, [rng.randrange(16)])
-        total += w.check()
-    assert total > 1000
+    workloads.random_mixed_batches(pcdn, seed, variant)
 
 
 def test_state_change_is_ordered_with_messages(pcdn):
@@ -257,27 +64,7 @@ def test_state_change_is_ordered_with_messages(pcdn):
 def test_direct_hot_recipient_keeps_order(pcdn):
     """many directs to ONE key in one batch (votes to a leader): per-connection order = batch order
     (R9) — exercises the stable (connection, message) sort"""
-    rng = random.Random(7)
-    w = World(pcdn, max_conns=20480, max_keys=65536, max_batch_msgs=8192, ring_bytes_per_conn=1 << 20,
-              max_batch_bytes=8 << 20)
-    keys = [rng.getrandbits(128).to_bytes(16, "little") * 8 for _ in range(20000)]  # 128-byte keys
-    for k in keys:
-        w.add_user(k, [0] if rng.random() < 0.001 else [])
-    leader = keys[123]
-    for j in range(6000):
-        r = rng.random()
-        if r < 0.5:
-            rc = leader
-        elif r < 0.9:
-            rc = rng.choice(keys)
-        else:
-            rc = rng.getrandbits(128).to_bytes(16, "little") * 8  # unknown: dropped
-        w.direct(rc, orc.direct_frame(rc, j.to_bytes(4, "little") * rng.randrange(1, 30)))
-        if j % 500 == 0:
-            w.bcast([0], orc.broadcast_frame([0], b"tick%d" % j))
-    n = w.check()
-    assert n > 5000
-    assert w.e.last_result.n_direct_dropped > 300
+    workloads.direct_hot_recipient_keeps_order(pcdn)
 
 
 def test_ring_wrap_and_release(pcdn):
@@ -390,7 +177,7 @@ def test_global_memory_pool_backpressure(pcdn):
         w.e.handle_broadcast_message([0], raw)
     with pytest.raises(pcdn.PcdnError) as ei:
         w.e.handle_broadcast_message([0], raw)         # 4 x 3056 > 10 000
-    assert ei.value.code == -11                        # PCDN_EAGAIN: the reference would await the semaphore
+    assert ei.value.code == PCDN_EAGAIN               # the reference would await the semaphore
     assert w.e.stats().inflight_bytes == 3 * len(raw)
     assert w.e.next_batch() != 0 and w.e.stats().batches == 1   # the refusal launched the open batch (no flush yet)
     got = w.e.drain()                                  # poll + release → permits returned
@@ -469,7 +256,7 @@ def test_concurrent_ingest_and_egress_threads(pcdn):
     for i, (sender, raw) in enumerate(frames):
         while True:
             rc = w.e.user_receive(sender, raw)
-            if rc != -11:          # PCDN_EAGAIN: all batch slots in flight — the consumer will free one
+            if rc != PCDN_EAGAIN:  # all batch slots in flight — the consumer will free one
                 break
             time.sleep(0.0002)
         assert rc == 0
@@ -522,7 +309,7 @@ def test_connection_id_quarantined_until_batches_released(pcdn):
     b1 = e.flush()
     with pytest.raises(pcdn.PcdnError) as ei:
         e.add_user(A, [0])
-    assert ei.value.code == -11            # PCDN_EAGAIN
+    assert ei.value.code == PCDN_EAGAIN
     assert e.num_users()[0] == 2           # refused before the kick: A is still connected
     e.poll(b1); e.release_batch(b1)
     e.add_user(A, [0])                     # now the kick + re-add goes through

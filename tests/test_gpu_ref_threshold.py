@@ -4,88 +4,26 @@ framed copy, in the same span and in batch order.  What a writer emits from eith
 oracle's stream; the records must be exactly the documented layouts; and a message far larger than a ring
 must reach every recipient without an overflow.
 
-Several tests run existing test bodies unchanged on engines created with a threshold (MixedPcdn): their
-frames run from 0 B to 40 KB, so every batch mixes both kinds of record."""
+Several tests run existing workloads (gpu_workloads) with delivery=("ref", T): their frames run from 0 B to
+40 KB, so every batch mixes both kinds of record."""
 import ctypes as C
 import os
 import random
-import struct
 
 import pytest
 
+import gpu_workloads as workloads
+from gpu_world import PCDN_EINVAL, STATUS_EAGAIN, World, chunk_streams, payload, records, shard_cfg, wire
 from kconst import K
-import test_gpu_device_parse as device_parse_tests
-import test_gpu_egress as egress_tests
-import test_gpu_egress_backlog as backlog_tests
-import test_gpu_inbatch_subscribe as inbatch_tests
-import test_gpu_parity as parity_tests
-import test_gpu_pool_retry as pool_tests
 from oracle import oracle as orc
-from test_gpu_egress import wire
-from test_gpu_parity import World, payload, shard_cfg
-from test_gpu_shared_payload import ref_record
 
 pytestmark = pytest.mark.gpu
 
-EINVAL = -1
-EAGAIN = 11          # pcdn_batch_result.status of a batch refused for space
-RING_DEFAULT = 1 << 16   # pcdn_config_default: ring_bytes_per_conn (and max_conns)
+MIXED = ("ref", 2048)
 
 
-def largest_threshold(cap):
-    """the largest ref_min_bytes an engine whose ring (or pool) holds `cap` bytes admits: the largest copied
-    record, round_up(4 + T - 1, 32), must fit it"""
-    return cap - 3
-
-
-class MixedPcdn:
-    """the package, with ref_min_bytes set on every engine it creates: `threshold`, or the largest value
-    the engine's ring (pool) admits when that is smaller"""
-
-    def __init__(self, pcdn, threshold=2048):
-        self._p = pcdn
-        self.threshold = threshold
-
-    def __getattr__(self, name):
-        return getattr(self._p, name)
-
-    def Engine(self, **kw):
-        fl = kw.get("flags", 0)
-        cap = kw.get("ring_bytes_per_conn", RING_DEFAULT)
-        if fl & self._p.FLAG_OUTPUT_POOL:
-            cap = kw.get("pool_bytes") or kw.get("max_conns", RING_DEFAULT) * cap
-        kw["ref_min_bytes"] = min(self.threshold, largest_threshold(cap))
-        return self._p.Engine(**kw)
-
-
-def walk(data, n_records):
-    """the records of a span: ('copy', raw) or ('ref', raw length, offset, batch id), and the record bytes"""
-    out, p = [], 0
-    for _ in range(n_records):
-        L = int.from_bytes(data[p:p + 4], "big")
-        if L == 0xFFFFFFFF:
-            L = int.from_bytes(data[p + 4:p + 8], "big")
-            off, bid = struct.unpack("<QQ", data[p + 8:p + 24])
-            out.append(("ref", L, off, bid, data[p:p + 32]))
-            p += 32
-        else:
-            out.append(("copy", data[p + 4:p + 4 + L]))
-            p += (4 + L + 31) // 32 * 32
-    assert p == len(data), (p, len(data))
-    return out
-
-
-def mixed_streams(chunk, out, payload_base, batch_id):
-    """an egress chunk's spans, both kinds of record, as wire bytes per connection"""
-    for i in range(chunk.n_spans):
-        sp = chunk.spans[i]
-        for r in walk(C.string_at(chunk.data + chunk.data_off[i], sp.len), sp.n_records):
-            if r[0] == "copy":
-                fr = r[1]
-            else:
-                assert r[3] == batch_id
-                fr = C.string_at(payload_base + r[2], r[1])
-            out.setdefault(sp.conn, bytearray()).extend(len(fr).to_bytes(4, "big") + fr)
+def kinds(recs):
+    return ["copy" if isinstance(r, bytes) else "ref" for r in recs]
 
 
 def read_span(e, res, conn, off, ln, hb, ring_bytes, pool=False):
@@ -98,24 +36,23 @@ def read_span(e, res, conn, off, ln, hb, ring_bytes, pool=False):
 
 
 # ------------------------------------------------------------------ 1. existing bodies on mixed engines
-@pytest.mark.parametrize("variant", [0, "staged", "runs", "runs-staged", "pool", "pool-staged-runs", "pool-host", "pool-shards", "pool-shards-nccl",
-                                     "pool-shards-staged", "host", "shards-host", "shards-host-staged", "shards-nccl"])
+@pytest.mark.parametrize("variant", workloads.MIXED_LAYOUTS)
 @pytest.mark.parametrize("seed", [0, 1])
 def test_random_mixed_batches_mixed(pcdn, seed, variant):
     """the randomized workload (frames 0 B .. 40 KB, local / remote / unknown directs, state changes between
     batches) with messages of >= 2048 bytes delivered by reference, on every layout"""
-    parity_tests.test_random_mixed_batches(MixedPcdn(pcdn), seed, variant)
+    workloads.random_mixed_batches(pcdn, seed, variant, delivery=MIXED)
 
 
 @pytest.mark.parametrize("seed", [0, 2])
 def test_device_parse_mixed(pcdn, seed):
     """device parse (seed 2: regular control kernels): a frame with a non-zero msg_status writes no record"""
-    device_parse_tests.test_frames_through_receive_loops(MixedPcdn(pcdn), seed)
+    workloads.frames_through_receive_loops(pcdn, seed, delivery=MIXED)
 
 
 @pytest.mark.parametrize("staged", [False, True])
 def test_device_parse_status_codes_mixed(pcdn, staged):
-    device_parse_tests.test_msg_status_codes(MixedPcdn(pcdn), staged)
+    workloads.msg_status_codes(pcdn, staged, delivery=MIXED)
 
 
 # (these bodies arrange their refusal with 100 KB copies that fill a 4 MiB pool: there the threshold sits
@@ -125,16 +62,16 @@ def test_device_parse_status_codes_mixed(pcdn, staged):
 @pytest.mark.parametrize("control", ["fused", "regular"])
 @pytest.mark.parametrize("layout", ["one-shard", "shards-host"])
 def test_pool_retry_routes_as_launched_mixed(pcdn, layout, control, runs):
-    pool_tests.test_retry_routes_as_launched(MixedPcdn(pcdn, threshold=1 << 17), layout, control, runs)
+    workloads.retry_routes_as_launched(pcdn, layout, control, runs, delivery=("ref", 1 << 17))
 
 
 def test_pool_partial_refusal_mixed(pcdn):
-    pool_tests.test_partial_refusal_across_shards(MixedPcdn(pcdn, threshold=1 << 17))
+    workloads.partial_refusal_across_shards(pcdn, delivery=("ref", 1 << 17))
 
 
 @pytest.mark.parametrize("how", ["write_batch", "soft_close"])   # (its "drain" sink walks framed records only)
 def test_pool_egress_refused_shard_written_once_mixed(pcdn, how):
-    pool_tests.test_egress_refused_shard_is_written_once(MixedPcdn(pcdn, threshold=1 << 17), how)
+    workloads.egress_refused_shard_is_written_once(pcdn, how, delivery=("ref", 1 << 17))
 
 
 @pytest.mark.parametrize("layout", ["one-shard", "shards-host"])
@@ -145,10 +82,10 @@ def test_pool_refusal_and_retry_with_references(pcdn, layout, control):
     follow, a later batch of a reference and a copy broadcast queues behind it.  After the releases the
     retried batches deliver what they would have delivered at launch, bit for bit against the oracle."""
     kw = dict(max_conns=1024, flags=pcdn.FLAG_OUTPUT_POOL | (pcdn.FLAG_STAGED_SPANS if control == "regular" else 0),
-              pool_bytes=8192, batch_slots=4, ref_min_bytes=16)
+              pool_bytes=8192, batch_slots=4)
     if layout == "shards-host":
         kw.update(shard_cfg(pcdn, layout))
-    w = World(pcdn, **kw)
+    w = World(pcdn, delivery=("ref", 16), **kw)
     keys = [b"user-%03d" % i for i in range(120)]
     conn = {k: w.add_user(k, [0]) for k in keys}
     hot = b"hot"
@@ -164,14 +101,14 @@ def test_pool_refusal_and_retry_with_references(pcdn, layout, control):
         w.direct(k, b"short copy")
     b1 = w.e.flush()
     assert w.e.poll(b0).status == 0
-    assert w.e.poll_shard(b1, home).status == EAGAIN
+    assert w.e.poll_shard(b1, home).status == STATUS_EAGAIN
     w.both("unsubscribe_user_from", on_home[0], [0])
     w.both("remove_user", on_home[1])
     w.add_user(b"newcomer", [0])
     w.bcast([0], b"after the changes, by reference")
     w.bcast([0], b"a copy")
     b2 = w.e.flush()
-    assert w.e.poll_shard(b2, home).status == EAGAIN
+    assert w.e.poll_shard(b2, home).status == STATUS_EAGAIN
     got = {}
     for b, retry in ((b0, False), (b1, True), (b2, True)):
         if retry:
@@ -185,12 +122,12 @@ def test_pool_refusal_and_retry_with_references(pcdn, layout, control):
     assert w.compare(w.e, got, w.expect()) > 240 + 2 * 110
 
 
-@pytest.mark.parametrize("variant", ["fused", "staged", "pool", "shards"])
-@pytest.mark.parametrize("case", [inbatch_tests.case_sub_around_broadcast, inbatch_tests.case_class_thresholds,
-                                  inbatch_tests.case_many_messages, inbatch_tests.case_wide], ids=lambda f: f.__name__[5:])
+@pytest.mark.parametrize("variant", [pytest.param("rings", id="fused"), "staged", "pool", pytest.param("shards-host", id="shards")])
+@pytest.mark.parametrize("case", [workloads.case_sub_around_broadcast, workloads.case_class_thresholds,
+                                  workloads.case_many_messages, workloads.case_wide], ids=lambda f: f.__name__[5:])
 def test_inbatch_subscribe_mixed(pcdn, case, variant):
     """in-batch subscription events on mixed engines (threshold 64: most broadcasts of these cases are references)"""
-    inbatch_tests.test_inbatch_subscribe(MixedPcdn(pcdn, threshold=64), case, variant)
+    workloads.inbatch_subscribe(pcdn, case, variant, delivery=("ref", 64))
 
 
 # ------------------------------------------------------------------ 2. exact records at the threshold
@@ -230,17 +167,17 @@ def test_records_at_the_threshold(pcdn, mode):
             i = conns.index(conn)
             mine = [m for m, x in enumerate(msgs)
                     if (x[0] == "b" and (x[1][0] == 0 or i < 10)) or (x[0] == "d" and x[1] == keys[i])]
-            recs = walk(read_span(e, res, conn, off, ln, hb, RB, mode == "pool"), nrec)
+            recs = records(read_span(e, res, conn, off, ln, hb, RB, mode == "pool"), nrec, b)
             assert len(recs) == len(mine) == nrec
             units = 0
             for m, r in zip(mine, recs):
                 raw = msgs[m][2]
                 if len(raw) < T:
-                    assert r == ("copy", raw)
+                    assert r == raw, (conn, m)
                     units += (4 + len(raw) + 31) // 32
                 else:
-                    assert r[0] == "ref" and r[4] == ref_record(len(raw), offs[m], b), (conn, m)
-                    assert C.string_at(base + r[2], len(raw)) == raw
+                    assert r == (len(raw), offs[m], b), (conn, m)
+                    assert C.string_at(base + r[1], len(raw)) == raw
                     units += 1
             assert ln == units * 32
             if mode == "pool":
@@ -265,14 +202,14 @@ def test_message_larger_than_a_ring(pcdn, mode):
     oracle's streams, and the 1 KiB messages sit in the rings as framed copies.  device: the batch goes
     through pcdn_submit_device"""
     T, N = 16 << 10, 4096
-    cfg = dict(max_conns=N, ring_bytes_per_conn=1 << 16, max_batch_bytes=24 << 20, max_batch_deliveries=1 << 16, ref_min_bytes=T)
+    cfg = dict(max_conns=N, ring_bytes_per_conn=1 << 16, max_batch_bytes=24 << 20, max_batch_deliveries=1 << 16)
     if mode == "pool":
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=64 << 20)
     if mode == "host-rings":
         cfg.update(flags=pcdn.FLAG_HOST_RINGS)
     if mode == "shards-host":
         cfg.update(shard_cfg(pcdn, mode), max_conns=2048)
-    w = World(pcdn, **cfg)
+    w = World(pcdn, delivery=("ref", T), **cfg)
     keys = [b"user-%05d" % i for i in range(N)]
     conns = [w.add_user(k, [0]) for k in keys]
     eg = pcdn.Egress(w.e, n_threads=8)
@@ -305,8 +242,8 @@ def test_message_larger_than_a_ring(pcdn, mode):
         if mode in ("rings", "host-rings"):
             for conn, off, ln, nrec in w.e.spans(res):
                 if conn == conns[1]:
-                    kinds = [r[0] for r in walk(read_span(w.e, res, conn, off, ln, hb, 1 << 16), nrec)]
-                    assert kinds == ["copy", "ref", "copy", "copy", "ref"], kinds
+                    got = kinds(records(read_span(w.e, res, conn, off, ln, hb, 1 << 16), nrec, b))
+                    assert got == ["copy", "ref", "copy", "copy", "ref"], got
         st = eg.write_batch(b)
         w.e.release_batch(b)
         exp = w.expect()
@@ -371,7 +308,7 @@ def test_class_and_launch_edges_low_threshold(pcdn, control):
     recipient sets; directs on both sides of T to local, remote and unknown keys; a batch of
     kThinSeparateMin directs (its own k_pack_direct launch) of both kinds — fused and regular control"""
     T = 1024
-    w = World(pcdn, max_conns=8192, ring_bytes_per_conn=1 << 18, ref_min_bytes=T,
+    w = World(pcdn, max_conns=8192, ring_bytes_per_conn=1 << 18, delivery=("ref", T),
               flags=pcdn.FLAG_STAGED_SPANS if control == "staged" else 0)
     rng = random.Random(9)
     N = 8192
@@ -448,11 +385,11 @@ def test_launch_count(pcdn, control):
 @pytest.mark.parametrize("mode", ["hbm", "host-rings", "shards-host", "pool-runs"])
 def test_writer_to_file_descriptors_mixed(pcdn, mode):
     """1100 memfds over six batches of 0 B .. 20 KB messages: each holds exactly the oracle's stream"""
-    egress_tests.test_writer_to_file_descriptors(MixedPcdn(pcdn), mode)
+    workloads.writer_to_file_descriptors(pcdn, mode, delivery=MIXED)
 
 
 def test_sockets_backpressure_failure_and_soft_close_mixed(pcdn):
-    egress_tests.test_sockets_backpressure_failure_and_soft_close(MixedPcdn(pcdn))
+    workloads.sockets_backpressure_failure_and_soft_close(pcdn, delivery=MIXED)
 
 
 @pytest.mark.parametrize("mode", ["hbm", "pool", "host-rings", "shards-host"])
@@ -465,18 +402,18 @@ def test_callback_sink_mixed(pcdn, mode):
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=256 << 20)
     if mode == "shards-host":
         cfg.update(shard_cfg(pcdn, mode), max_conns=1024)
-    w = World(MixedPcdn(pcdn), **cfg)
+    w = World(pcdn, delivery=MIXED, **cfg)
     eg = pcdn.Egress(w.e)
     rng = random.Random(4)
     keys = [rng.getrandbits(64).to_bytes(8, "little") * 2 for _ in range(1200)]
     for k in keys:
         w.add_user(k, [x for x in range(4) if rng.random() < 0.4])
     for rnd in range(4):
-        egress_tests.traffic(w, rng, keys, 60)
+        workloads.traffic(w, rng, keys, 60)
         b = w.e.flush()
         base = w.e.batch_payload(b)
         got = {}
-        eg.drain(b, lambda ch: mixed_streams(ch, got, base, b))
+        eg.drain(b, lambda ch: chunk_streams(ch, got, base, b))
         w.e.release_batch(b)
         assert {c: bytes(v) for c, v in got.items()} == {c: wire(fr) for c, fr in w.expect().items()}
     eg.close()
@@ -487,7 +424,7 @@ def test_callback_sink_mixed(pcdn, mode):
 def test_stalled_peer_gets_reference_payload_after_release(pcdn, mode):
     """a stalled peer's backlog holds the payload bytes of its reference records: the batches (and with
     batch_slots=2 their payload staging) are released and reused before the peer reads anything"""
-    backlog_tests.test_stalled_peer_does_not_stall_the_others(MixedPcdn(pcdn), mode)
+    workloads.stalled_peer_does_not_stall_the_others(pcdn, mode, delivery=MIXED)
 
 
 # ------------------------------------------------------------------ 7. configuration
@@ -495,7 +432,8 @@ def test_stalled_peer_gets_reference_payload_after_release(pcdn, mode):
 def test_old_config_size_is_a_copy_engine(pcdn):
     """a pcdn_config of the size before ref_min_bytes (struct_size = its offset) is a copy engine: the
     bytes behind that size are not read, so every record is a framed copy"""
-    w = World(pcdn, max_conns=1024, ring_bytes_per_conn=1 << 18, struct_size=pcdn.Config.ref_min_bytes.offset, ref_min_bytes=64)
+    # (asked for threshold 64, which the old struct size hides from pcdn_create)
+    w = World(pcdn, max_conns=1024, ring_bytes_per_conn=1 << 18, struct_size=pcdn.Config.ref_min_bytes.offset, delivery=("ref", 64))
     keys = [b"user%03d" % i for i in range(100)]
     for i, k in enumerate(keys):
         w.add_user(k, [i % 2])
@@ -506,13 +444,13 @@ def test_old_config_size_is_a_copy_engine(pcdn):
     res = w.e.poll(b)
     assert res.status == 0 and res.n_overflow == 0
     for conn, off, ln, nrec in w.e.spans(res):
-        assert all(r[0] == "copy" for r in walk(w.e.read(conn, off, ln), nrec))
+        assert kinds(records(w.e.read(conn, off, ln), nrec)) == ["copy"] * nrec, conn
     assert w.e.collect_frames(res) == w.expect()
     w.e.release_batch(b)
     w.e.close()
     with pytest.raises(pcdn.PcdnError) as ei:
         pcdn.Engine(max_conns=1024, struct_size=pcdn.Config.ref_min_bytes.offset - 8)
-    assert ei.value.code == EINVAL
+    assert ei.value.code == PCDN_EINVAL
 
 
 @pytest.mark.parametrize("variant", [0, "pool", "shards-host"])
@@ -546,7 +484,7 @@ def test_threshold_zero_is_the_copy_engine(pcdn, variant):
             assert res.status == 0 and res.n_overflow == 0
             pool = bool(e.cfg.flags & pcdn.FLAG_OUTPUT_POOL)
             for conn, off, ln, nrec in sorted(e.spans(res)):
-                recs = walk(e.read(conn, res.pool_base + off if pool else off, ln), nrec)
+                recs = records(e.read(conn, res.pool_base + off if pool else off, ln), nrec)
                 out.append((conn, off, ln, nrec, recs))
             out.append((res.n_deliveries, res.bytes_out, res.n_spans, res.pool_base))
             e.release_batch(b)

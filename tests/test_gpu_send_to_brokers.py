@@ -2,52 +2,23 @@
 messages of cdn-broker/src/tasks/broker/sync.rs) go to one peer broker or to every peer broker as one message
 of the open batch, in order with the routed traffic of the same link.  Every connection's stream is compared
 frame for frame with the oracle's, which sends them through try_send_to_broker(s) (tasks/broker/sender.rs:17-59,
-restated in test_send_to_brokers_host.py), on every span layout, both control paths, shards, device parse,
+restated in gpu_world.py and tested in test_send_to_brokers_host.py), on every span layout, both control paths, shards, device parse,
 in-batch subscription events, shared payload, a by-reference threshold, the output pool's refusal and retry, and
 the egress writer."""
 import random
 
 import pytest
 
+from gpu_world import (BIG, PCDN_EAGAIN, PCDN_ENOSPC, STATUS_EAGAIN, PoolWorld, Reader, Sends, World, flush_until_done,
+                       layout, payload, shard_cfg, sock_pair, user_sync, wire)
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_egress import wire
-from test_gpu_egress_backlog import BIG, Reader, flush_until_done, sock_pair
-from test_gpu_parity import World, payload, shard_cfg
-from test_gpu_pool_retry import EAGAIN, PoolWorld
-from test_send_to_brokers_host import try_send_to_broker, try_send_to_brokers
 
 pytestmark = pytest.mark.gpu
 
-ENOSPC, EAGAIN_RC = -5, -11
-LAYOUTS = ["rings", "staged", "runs", "host", "pool", "shards-host", "shards-nccl", "shared", "ref"]
-
-
-def layout_cfg(pcdn, layout):
-    if layout.startswith("shards"):
-        return shard_cfg(pcdn, layout)
-    return {"rings": {}, "staged": dict(flags=pcdn.FLAG_STAGED_SPANS), "runs": dict(flags=pcdn.FLAG_SPAN_RUNS),
-            "host": dict(flags=pcdn.FLAG_HOST_RINGS), "pool": dict(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=256 << 20),
-            "shared": dict(flags=pcdn.FLAG_SHARED_PAYLOAD), "ref": dict(ref_min_bytes=2048),
-            }[layout]
-
-
-class Sends:
-    """a World (or one of its subclasses) that also sends the broker's own frames: the engine's
-    pcdn_send_to_broker(s) against try_send_to_broker(s) on its oracle"""
-
-    def add_broker(self, ident, topics=()):
-        self.__dict__.setdefault("idents", []).append(ident)
-        return super().add_broker(ident, topics)
-
-    def send(self, ident, raw):
-        """send_to_broker(ident, raw), or send_to_brokers(raw) with ident None, on both; the results must agree"""
-        if ident is None:
-            r, ro = self._engine("send_to_brokers", raw), try_send_to_brokers(self.o, self.__dict__.get("idents", []), raw)
-        else:
-            r, ro = self._engine("send_to_broker", ident, raw), try_send_to_broker(self.o, ident, raw)
-        assert r == ro, (ident, r, ro)
-        return r
+# (layout, delivery) under this file's test ids
+LAYOUTS = [pytest.param(n, "copy", id=n) for n in ("rings", "staged", "runs", "host", "pool", "shards-host", "shards-nccl")] + \
+          [pytest.param("rings", "shared", id="shared"), pytest.param("rings", ("ref", 2048), id="ref")]
 
 
 class SendWorld(Sends, World):
@@ -56,10 +27,6 @@ class SendWorld(Sends, World):
 
 class SendPoolWorld(Sends, PoolWorld):
     pass
-
-
-def user_sync(tag, n=300):
-    return orc.serialize(orc.KIND_USER_SYNC, b"", bytes([tag % 256]) * n)
 
 
 def topic_sync(tag, n=40):
@@ -98,10 +65,13 @@ def connect_flow(w, rng, across, users_only, tag=0):
 
 
 @pytest.mark.parametrize("flow", ["one-batch", "across", "users-only"])
-@pytest.mark.parametrize("layout", LAYOUTS)
-def test_connect_flow(pcdn, layout, flow):
-    w = SendWorld(pcdn, max_conns=1024, **layout_cfg(pcdn, layout))
-    rng = random.Random(f"{layout}-{flow}")
+@pytest.mark.parametrize("name,delivery", LAYOUTS)
+def test_connect_flow(pcdn, request, name, delivery, flow):
+    cfg = layout(pcdn, name)
+    if name == "pool":
+        cfg["pool_bytes"] = 256 << 20
+    w = SendWorld(pcdn, max_conns=1024, delivery=delivery, **cfg)
+    rng = random.Random(request.node.callspec.id)          # seeded by the test id, "<layout>-<flow>"
     populate(w)
     connect_flow(w, rng, flow == "across", flow == "users-only")
     assert w.check() > 0
@@ -201,7 +171,7 @@ def test_pool_retry_delivers_to_the_set_at_launch(pcdn, control):
     assert w.send(None, user_sync(7, 20000)) == 0
     assert w.send("r/s", topic_sync(7)) == 0
     b1 = w.traffic(1, (w.keys[0],))
-    assert w.e.poll(b0).status == 0 and w.e.poll(b1).status == EAGAIN
+    assert w.e.poll(b0).status == 0 and w.e.poll(b1).status == STATUS_EAGAIN
     w.both("remove_broker", "p/q")
     w.add_broker("t/u", [0])
     got = {}
@@ -277,7 +247,7 @@ def test_overflow_in_copy_mode(pcdn):
 def test_by_reference_threshold(pcdn):
     """ref_min_bytes = T: a sync frame >= T and larger than a ring is delivered by reference without an
     overflow, one below T is framed"""
-    w = SendWorld(pcdn, max_conns=64, ring_bytes_per_conn=1 << 16, ref_min_bytes=4096)
+    w = SendWorld(pcdn, max_conns=64, ring_bytes_per_conn=1 << 16, delivery=("ref", 4096))
     w.add_broker("b/b")
     w.add_user(b"u", [0])
     assert w.send(None, user_sync(1, 200_000)) == 0
@@ -299,7 +269,7 @@ def test_counters_and_memory_pool(pcdn):
     w.bcast([0], routed)
     with pytest.raises(pcdn.PcdnError) as ei:
         w.e.handle_broadcast_message([0], routed)
-    assert ei.value.code == EAGAIN_RC
+    assert ei.value.code == PCDN_EAGAIN
     s = w.send(None, user_sync(1, 30_000))            # larger than the whole pool: no permits taken
     assert s == 0
     st = w.e.stats()
@@ -322,7 +292,7 @@ def test_full_batch_and_too_large(pcdn):
     assert w.e.stats().batches == 1
     with pytest.raises(pcdn.PcdnError) as ei:
         w.e.send_to_brokers(b"q" * (1 << 16))
-    assert ei.value.code == ENOSPC
+    assert ei.value.code == PCDN_ENOSPC
     w.check()
     assert w.e.stats().msgs == 5 and w.e.stats().batches == 2
     w.e.close()

@@ -3,16 +3,15 @@ against ONE unsharded oracle, stream for stream.  'shards-host' puts the shards 
 one-GPU box); 'shards-nccl' uses one GPU per shard and the library's own ncclBroadcast ingest (needs
 >= 2 GPUs).  The randomized mixed workload on sharded engines lives in
 test_gpu_parity.py::test_random_mixed_batches[shards-*]."""
-import ctypes as C
 import random
 
-import numpy as np
 import pytest
 
+import gpu_workloads as workloads
 import scenarios
+from gpu_world import World, payload, shard_cfg
 from harness import EngineBackend
 from oracle import oracle as orc
-from test_gpu_parity import World, payload, shard_cfg
 
 pytestmark = pytest.mark.gpu
 
@@ -79,62 +78,7 @@ def test_shards_balance_counters_and_per_shard_results(pcdn, variant):
 def test_sharded_device_resident_batch(pcdn, variant):
     """pcdn_submit_device on a sharded engine: the batch lies on the root GPU (global shard 0) and the
     library replicates frames + descriptors to the other shards (NCCL broadcast / peer copies)."""
-    import torch
-
-    w = World(pcdn, max_conns=2048, ring_bytes_per_conn=1 << 16, max_batch_bytes=1 << 20, **shard_cfg(pcdn, variant))
-    rng = random.Random(3)
-    keys = [rng.getrandbits(64).to_bytes(8, "little") * 4 for _ in range(1000)]
-    for i, k in enumerate(keys):
-        w.add_user(k, [i % 3])
-    M = 12
-    frames, kinds, topics, aux_off, aux_len = [], [], [], [], []
-    arena = bytearray()
-    slot_off = []
-    for m in range(M):
-        if m % 4 == 3:
-            rc = keys[m * 17]
-            fr = orc.direct_frame(rc, payload(rng, 100 + m))
-            w.o.handle_direct_message(rc, fr, False)
-            kinds.append(3)
-        else:
-            t = [m % 3]
-            fr = orc.broadcast_frame(t, payload(rng, 500 * m + 1))
-            w.o.handle_broadcast_message(t, fr, False)
-            kinds.append(4)
-        slot_off.append(len(arena) // 16)
-        arena += bytes(4) + fr + bytes((-(4 + len(fr))) % 16)
-        if kinds[-1] == 3:
-            aux_off.append(len(arena)); aux_len.append(len(rc))
-            arena += rc + bytes((-len(rc)) % 16)
-        else:
-            aux_off.append(len(topics)); aux_len.append(1)
-            topics.append(m % 3)
-        frames.append(fr)
-    dev = torch.device("cuda", w.e.shard_info(0).device)
-    t8 = lambda a: torch.tensor(list(a), dtype=torch.uint8, device=dev)
-    t32 = lambda a: torch.tensor(list(a), dtype=torch.int32, device=dev)
-    d_arena = t8(arena + bytes(64))
-    d_kind, d_flags = t8(kinds), t8([0] * M)
-    d_slot, d_len, d_aoff, d_alen = t32(slot_off), t32([len(f) for f in frames]), t32(aux_off), t32(aux_len)
-    d_topics = torch.tensor(topics, dtype=torch.int16, device=dev)
-    bidx = [i for i in range(M) if kinds[i] == 4]
-    d_bidx = t32(bidx)
-    torch.cuda.synchronize(dev)
-    db = pcdn.DeviceBatch(M, len(bidx), d_arena.data_ptr(), len(arena), d_kind.data_ptr(), d_flags.data_ptr(), d_slot.data_ptr(),
-                          d_len.data_ptr(), d_aoff.data_ptr(), d_alen.data_ptr(), d_topics.data_ptr(), len(topics), d_bidx.data_ptr())
-    for _ in range(3):   # slots are reused: the ingest regions must be rewritten correctly each time
-        b = w.e.submit_device(db)
-        res = w.e.poll(b)
-        assert res.status == 0
-        got = w.e.collect_frames(res)
-        w.e.release_batch(b)
-        assert got == w.expect()
-        for m in range(M):
-            if kinds[m] == 3:
-                w.o.handle_direct_message(keys[m * 17], frames[m], False)
-            else:
-                w.o.handle_broadcast_message([m % 3], frames[m], False)
-    w.e.close()
+    workloads.sharded_device_resident_batch(pcdn, variant)
 
 
 @pytest.mark.parametrize("variant", VARIANTS)

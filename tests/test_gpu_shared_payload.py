@@ -3,8 +3,8 @@ and the payload exists once per batch in pinned host memory (pcdn_batch_payload)
 from the records — p[4..8) then the L payload bytes — must be exactly the oracle's stream, on every
 layout the copy mode supports, and the records themselves must be bit for bit the documented layout.
 
-Several tests run the copy-mode test bodies unchanged on engines created with the flag (SharedPcdn):
-the streams they compare are the same, only the records in between differ."""
+Several tests run the copy-mode workloads (gpu_workloads) with delivery="shared": the streams they compare are
+the same, only the records in between differ."""
 import ctypes as C
 import os
 import random
@@ -13,72 +13,42 @@ import struct
 import numpy as np
 import pytest
 
-import test_gpu_device_parse as device_parse_tests
-import test_gpu_egress as egress_tests
-import test_gpu_parity as parity_tests
-import test_gpu_shards as shard_tests
+import gpu_workloads as workloads
+from gpu_world import STATUS_EAGAIN, PCDN_ENOENT, PCDN_ENOSPC, World, frames, payload, records, ref_record, shard_cfg, wire
 from oracle import oracle as orc
-from test_gpu_egress import wire
-from test_gpu_parity import World, payload, shard_cfg
 
 pytestmark = pytest.mark.gpu
-
-EAGAIN = 11
-
-
-class SharedPcdn:
-    """the package, with FLAG_SHARED_PAYLOAD added to every engine it creates"""
-
-    def __init__(self, pcdn):
-        self._p = pcdn
-
-    def __getattr__(self, name):
-        return getattr(self._p, name)
-
-    def Engine(self, **kw):
-        kw["flags"] = kw.get("flags", 0) | self._p.FLAG_SHARED_PAYLOAD
-        return self._p.Engine(**kw)
-
-
-def ref_record(raw_len, off, batch_id):
-    """the model of a reference record (include/pcdn_fanout.h)"""
-    return b"\xff\xff\xff\xff" + raw_len.to_bytes(4, "big") + struct.pack("<QQ", off, batch_id) + bytes(8)
 
 
 def resolve(data, n_records, payload_base, batch_id):
     """the frames a writer emits for a span of reference records"""
-    out = []
-    for r in range(n_records):
-        p = r * 32
-        assert data[p:p + 4] == b"\xff\xff\xff\xff"
-        L = int.from_bytes(data[p + 4:p + 8], "big")
-        off, bid = struct.unpack("<QQ", data[p + 8:p + 24])
-        assert bid == batch_id and data[p + 24:p + 32] == bytes(8)
-        out.append(C.string_at(payload_base + off, L))
-    return out
+    recs = records(data, n_records, batch_id)
+    assert all(isinstance(r, tuple) for r in recs), "a shared-payload span holds a framed copy"
+    return frames(recs, payload_base)
 
 
 # ------------------------------------------------------------------ 1. randomized mixed workload
-@pytest.mark.parametrize("variant", [0, "staged", "runs", "pool", "pool-staged-runs", "host", "pool-host", "shards-host-staged"])
+@pytest.mark.parametrize("variant", [pytest.param("rings", id="0"), "staged", "runs", "pool", "pool-staged-runs", "host", "pool-host",
+                                     "shards-host-staged"])
 @pytest.mark.parametrize("seed", [0, 1])
 def test_random_mixed_batches_shared(pcdn, seed, variant):
     """the copy-mode randomized workload (frames 0 B .. 40 KB, local / remote / unknown directs, state
     changes between batches) with every delivery by reference: rings (0: the fused k_ctrl_small path of
     a small engine; staged: the regular control kernels), run-length spans, pool, pool + run-length spans,
     host rings, pool in host memory, three shards on GPU 0 with the regular control kernels"""
-    parity_tests.test_random_mixed_batches(SharedPcdn(pcdn), seed, variant)
+    workloads.random_mixed_batches(pcdn, seed, variant, delivery="shared")
 
 
 @pytest.mark.parametrize("seed", [0, 2])
 def test_device_parse_shared(pcdn, seed):
     """device parse (seed 2: with the regular control kernels): a frame with a non-zero msg_status
     writes no record; everything else is delivered by reference"""
-    device_parse_tests.test_frames_through_receive_loops(SharedPcdn(pcdn), seed)
+    workloads.frames_through_receive_loops(pcdn, seed, delivery="shared")
 
 
 @pytest.mark.parametrize("staged", [False, True])
 def test_device_parse_status_codes_shared(pcdn, staged):
-    device_parse_tests.test_msg_status_codes(SharedPcdn(pcdn), staged)
+    workloads.msg_status_codes(pcdn, staged, delivery="shared")
 
 
 # ------------------------------------------------------------------ 2. exact record bytes
@@ -122,7 +92,7 @@ def test_reference_record_bytes(pcdn, mode):
         e.release_batch(b)
         with pytest.raises(pcdn.PcdnError) as ei:
             e.batch_payload(b)
-        assert ei.value.code == -10                      # released: PCDN_ENOENT
+        assert ei.value.code == PCDN_ENOENT              # released
     e.close()
 
 
@@ -134,7 +104,7 @@ def test_large_messages_to_many_users(pcdn, out):
     cfg = dict(max_conns=4096, ring_bytes_per_conn=1 << 16, max_batch_bytes=24 << 20, max_batch_deliveries=1 << 16)
     if out == "pool":
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=1 << 20)
-    w = World(SharedPcdn(pcdn), **cfg)
+    w = World(pcdn, delivery="shared", **cfg)
     keys = [b"user-%05d" % i for i in range(4096)]
     conns = [w.add_user(k, [0]) for k in keys]
     eg = pcdn.Egress(w.e, n_threads=8)
@@ -178,13 +148,13 @@ def test_large_messages_to_many_users(pcdn, out):
 @pytest.mark.parametrize("mode", ["hbm", "host-rings", "shards-host", "pool-runs"])
 def test_writer_to_file_descriptors_shared(pcdn, mode):
     """1100 memfds over six batches: each holds exactly the oracle's stream"""
-    egress_tests.test_writer_to_file_descriptors(SharedPcdn(pcdn), mode)
+    workloads.writer_to_file_descriptors(pcdn, mode, delivery="shared")
 
 
 def test_sockets_backpressure_failure_and_soft_close_shared(pcdn):
     """a 4 KiB send buffer and a slow reader split writes between a record's 4 header bytes and its
     payload; a dead peer is reported once; soft_close still writes the open batch"""
-    egress_tests.test_sockets_backpressure_failure_and_soft_close(SharedPcdn(pcdn))
+    workloads.sockets_backpressure_failure_and_soft_close(pcdn, delivery="shared")
 
 
 @pytest.mark.parametrize("mode", ["hbm-small-chunks", "pool", "host-rings", "shards-host"])
@@ -198,14 +168,14 @@ def test_callback_sink_resolves_through_batch_payload(pcdn, mode):
         cfg.update(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=64 << 20)
     if mode == "shards-host":
         cfg.update(shard_cfg(pcdn, mode), max_conns=1024)
-    w = World(SharedPcdn(pcdn), **cfg)
+    w = World(pcdn, delivery="shared", **cfg)
     eg = pcdn.Egress(w.e, chunk_bytes=(1 << 17) if mode == "hbm-small-chunks" else 0)
     rng = random.Random(4)
     keys = [rng.getrandbits(64).to_bytes(8, "little") * 2 for _ in range(1200)]
     for k in keys:
         w.add_user(k, [x for x in range(4) if rng.random() < 0.4])
     for rnd in range(4):
-        egress_tests.traffic(w, rng, keys, 60)
+        workloads.traffic(w, rng, keys, 60)
         b = w.e.flush()
         base = w.e.batch_payload(b)
         got = {}
@@ -236,7 +206,7 @@ def test_pool_refusal_and_retry_shared(pcdn, layout, control):
               pool_bytes=8192, batch_slots=4)
     if layout == "shards-host":
         kw.update(shard_cfg(pcdn, layout))
-    w = World(SharedPcdn(pcdn), **kw)
+    w = World(pcdn, delivery="shared", **kw)
     keys = [b"user-%03d" % i for i in range(120)]
     conn = {k: w.add_user(k, [0]) for k in keys}
     hot = b"hot"
@@ -252,13 +222,13 @@ def test_pool_refusal_and_retry_shared(pcdn, layout, control):
         w.direct(k, orc.direct_frame(k, b"direct in the refused batch"))
     b1 = w.e.flush()
     assert w.e.poll(b0).status == 0
-    assert w.e.poll_shard(b1, home).status == EAGAIN
+    assert w.e.poll_shard(b1, home).status == STATUS_EAGAIN
     w.both("unsubscribe_user_from", on_home[0], [0])
     w.both("remove_user", on_home[1])
     w.add_user(b"newcomer", [0])
     w.bcast([0], orc.broadcast_frame([0], b"after the changes"))
     b2 = w.e.flush()
-    assert w.e.poll_shard(b2, home).status == EAGAIN
+    assert w.e.poll_shard(b2, home).status == STATUS_EAGAIN
     got = {}
 
     def consume(b, retry):
@@ -287,12 +257,12 @@ def test_pool_refusal_and_retry_shared(pcdn, layout, control):
 # ------------------------------------------------------------------ 6. direct paths
 def test_direct_hot_recipient_keeps_order_shared(pcdn):
     """thousands of directs to one key in one batch (> kHotMin hits, >= kThinSeparateMin directs)"""
-    parity_tests.test_direct_hot_recipient_keeps_order(SharedPcdn(pcdn))
+    workloads.direct_hot_recipient_keeps_order(pcdn, delivery="shared")
 
 
 def test_sharded_device_resident_batch_shared(pcdn):
     """pcdn_submit_device on three shards of GPU 0: the payload comes from the first shard's ingest region"""
-    shard_tests.test_sharded_device_resident_batch(SharedPcdn(pcdn), "shards-host")
+    workloads.sharded_device_resident_batch(pcdn, "shards-host", delivery="shared")
 
 
 @pytest.mark.parametrize("ready", [False, True])
@@ -302,7 +272,7 @@ def test_device_resident_batch_payload(pcdn, ready):
     staging, a larger one is ENOSPC"""
     import torch
 
-    w = World(SharedPcdn(pcdn), max_conns=2048, max_batch_bytes=1 << 20)
+    w = World(pcdn, max_conns=2048, max_batch_bytes=1 << 20, delivery="shared")
     rng = random.Random(6)
     keys = [b"k%07d" % i for i in range(600)]
     for i, k in enumerate(keys):
@@ -382,7 +352,7 @@ def test_device_resident_batch_payload(pcdn, ready):
     for arena_bytes in (cap + 16, (1 << 20) + 4096):
         with pytest.raises(pcdn.PcdnError) as ei:
             w.e.submit_device(sized(d_full.data_ptr(), arena_bytes))
-        assert ei.value.code == -5                      # PCDN_ENOSPC, nothing launched
+        assert ei.value.code == PCDN_ENOSPC             # nothing launched
         assert w.e.next_batch() == 0
     w.e.close()
 

@@ -7,12 +7,10 @@ import random
 
 import pytest
 
+from gpu_world import PCDN_EAGAIN, PCDN_ENOSPC, World
 from oracle import oracle as orc
-from test_gpu_parity import World
 
 pytestmark = pytest.mark.gpu
-
-ENOSPC, EAGAIN = -5, -11
 
 
 def _staged(msgs, max_key_len):
@@ -71,20 +69,20 @@ def test_explicit_batch_refusals(pcdn):
         assert left >= 32 and left % 16 == 0
         return base + [("b", [7], bytes([7]) * (left - 4), False)]
 
-    _refused(pcdn, w, filled(16), ENOSPC)
+    _refused(pcdn, w, filled(16), PCDN_ENOSPC)
     assert _staged(filled(0), KL) == B - 64
     _submit_both(w, filled(0))
     assert w.check() > 12
 
     small = [("b", [t], orc.broadcast_frame([t], b"s%d" % t), False) for t in range(MB + 1)]
-    _refused(pcdn, w, small, ENOSPC)
+    _refused(pcdn, w, small, PCDN_ENOSPC)
     _submit_both(w, small[:MB])
     assert w.check() > 0
 
     cap = 4 * M + 4096
     many = [list(range(256)) * 10, list(range(256)) * 10]           # 2 x 2560 = cap entries
     assert sum(map(len, many)) == cap
-    _refused(pcdn, w, [("b", many[0] + [1], b"t0", False), ("b", many[1], b"t1", False)], ENOSPC)
+    _refused(pcdn, w, [("b", many[0] + [1], b"t0", False), ("b", many[1], b"t1", False)], PCDN_ENOSPC)
     _submit_both(w, [("b", many[0], b"t0", False), ("b", many[1], b"t1", False)])
     assert w.check() > 0
     assert w.e.stats().inflight_bytes == 0
@@ -94,7 +92,7 @@ def test_explicit_batch_refusals(pcdn):
     first = [("b", [0], b"x" * 5000, False)]
     bid = _submit_both(p, first)
     second = [("b", [0], b"y" * 3000, False), ("d", b"a" * 8, b"z" * 3000, False)]
-    _refused(pcdn, p, second, EAGAIN)
+    _refused(pcdn, p, second, PCDN_EAGAIN)
     assert p.e.stats().inflight_bytes == 5000
     res = p.e.poll(bid)
     assert p.e.collect_frames(res) == p.expect()
@@ -139,10 +137,10 @@ def _receive_all(pcdn, e, frames, batched):
         else:
             s, o, raw = frames[pos]
             rcs[pos] = e.broker_receive("b0/p0", raw) if o else e.user_receive(s, raw)
-            done = EAGAIN if rcs[pos] == EAGAIN else 1
-        assert done == EAGAIN or done > 0
+            done = PCDN_EAGAIN if rcs[pos] == PCDN_EAGAIN else 1
+        assert done == PCDN_EAGAIN or done > 0
         pos += max(done, 0)
-        if pos < n and (done == EAGAIN or batched):
+        if pos < n and (done == PCDN_EAGAIN or batched):
             stops += 1
             before = len(sizes)
             _run_batches(e, sizes, out, flush=False)
@@ -266,7 +264,7 @@ def test_topic_overflow_frame_in_threaded_call(pcdn):
         sender = rng.choice(keys)
         if j == 1500:
             frames.append((sender, 0, big))
-            want_rc.append(ENOSPC)
+            want_rc.append(PCDN_ENOSPC)
             continue
         if rng.random() < 0.5:
             raw = orc.broadcast_frame([rng.randrange(2)], bytes([j & 255]) * rng.randrange(0, 300))
@@ -281,4 +279,4 @@ def test_topic_overflow_frame_in_threaded_call(pcdn):
     assert set(got) == set(want)
     for c in want:
         assert got[c] == want[c], c
-    assert w.e.user_receive(keys[0], big) == ENOSPC
+    assert w.e.user_receive(keys[0], big) == PCDN_ENOSPC

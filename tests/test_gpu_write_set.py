@@ -15,18 +15,14 @@ import random
 import numpy as np
 import pytest
 
-import test_gpu_cm_runs as cm_runs
-import test_gpu_kernel_edges as kedges
-import test_gpu_parity as parity
+import gpu_workloads as workloads
+from gpu_world import (CM_DENSE, CM_IDS, CM_MODES, CM_RING, EDGE_SLOTS, PCDN_ENOENT, STATUS_E2BIG, STATUS_EAGAIN, World,
+                       check, cm_frame, cm_world, edge_sizes, edge_world, layout, payload, raw, shard_cfg, span_table, units)
 from kconst import K
 from oracle import oracle as orc
-from test_gpu_kernel_edges import EDGE_SLOTS, edge_sizes, edge_world, raw, span_table, units
-from test_gpu_parity import World, payload, shard_cfg
 
 pytestmark = pytest.mark.gpu
 
-EAGAIN, E2BIG = 11, 12          # pcdn_batch_result.status of a refused batch
-ENOENT = -10
 CHUNK_WORDS = 1 << 24           # canary generated / compared 128 MiB at a time
 M64 = (1 << 64) - 1
 
@@ -45,7 +41,8 @@ class _Cuda:
 
 class Guard:
     """the canary over every local shard's output memory, and the record of every batch polled since
-    it was last filled (per shard: status, pool_base, expanded span table, placement / release time)"""
+    it was last filled (per shard: status, pool_base, expanded span table, placement / release time);
+    `verified` counts the drained cycles whose write set it checked"""
 
     def __init__(self, pcdn, e):
         import torch
@@ -74,6 +71,7 @@ class Guard:
         self.clock = 0
         self.batches = {}           # batch id -> Rec, since the last fill
         self.launched = {}          # batch id -> clock at launch (batches launched through launch())
+        self.verified = 0
         self.fill()
 
     def tick(self):
@@ -184,7 +182,7 @@ class Guard:
             try:
                 self.e.poll(b)
             except Exception as ex:
-                if getattr(ex, "code", None) == ENOENT:
+                if getattr(ex, "code", None) == PCDN_ENOENT:
                     break
                 raise
             self.record(b, t0)
@@ -207,6 +205,7 @@ class Guard:
                 if len(live) > 1:
                     m = int(self.coverage(li, live).max())
                     assert m <= 1, f"spans of batches {[q.bid for q in live]}, unreleased together, overlap on shard {li}"
+        self.verified += 1
         self.fill()
 
 
@@ -246,12 +245,12 @@ class GuardedWorld(World):
         rec = g.record(b, t0)
         if res.status:
             g.refused(rec, t0)
-        if res.status == EAGAIN:
+        if res.status == STATUS_EAGAIN:
             self.refusals += 1
             e.retry_batch(b)
             t = g.tick()
             for s in rec.shards:
-                if s.status == EAGAIN:
+                if s.status == STATUS_EAGAIN:
                     s.placed = t
             res = e.poll(b)
             rec = g.record(b, t0)
@@ -296,40 +295,25 @@ class GuardedWorld(World):
         return t[t[:, 0] == conn][:, 1:].tolist()
 
 
-@pytest.fixture
-def guarded(monkeypatch):
-    """run another test module's workload with its World replaced by GuardedWorld"""
-
-    def use(*modules):
-        for m in modules:
-            monkeypatch.setattr(m, "World", GuardedWorld)
-
-    return use
-
-
-
-
 # ------------------------------------------------------------------ the guard around existing workloads
-EDGE_MODES = ["rings-fused", "rings-regular", "pool-fused", "pool-regular", "runs", "shared-payload", "ref-min"]
+# (layout, delivery) under this file's test ids
+EDGE_MODES = [pytest.param("rings", "copy", id="rings-fused"), pytest.param("staged", "copy", id="rings-regular"),
+              pytest.param("pool", "copy", id="pool-fused"), pytest.param("pool-staged", "copy", id="pool-regular"),
+              pytest.param("runs", "copy", id="runs"), pytest.param("rings", "shared", id="shared-payload"),
+              pytest.param("rings", ("ref", 12000), id="ref-min")]
 
 
-def edge_cfg(pcdn, mode):
-    return {"rings-fused": dict(), "rings-regular": dict(flags=pcdn.FLAG_STAGED_SPANS),
-            "pool-fused": dict(flags=pcdn.FLAG_OUTPUT_POOL, pool_bytes=1 << 30),
-            "pool-regular": dict(flags=pcdn.FLAG_OUTPUT_POOL | pcdn.FLAG_STAGED_SPANS, pool_bytes=1 << 30),
-            "runs": dict(flags=pcdn.FLAG_SPAN_RUNS), "shared-payload": dict(flags=pcdn.FLAG_SHARED_PAYLOAD),
-            "ref-min": dict(ref_min_bytes=12000)}[mode]
-
-
-@pytest.mark.parametrize("mode", EDGE_MODES)
-def test_size_and_recipient_classes_under_guard(pcdn, guarded, mode):
+@pytest.mark.parametrize("name,delivery", EDGE_MODES)
+def test_size_and_recipient_classes_under_guard(pcdn, name, delivery):
     """every raw length of edge_sizes() to every recipient count of recipient_counts(): thin, message-major
     (tile edges), dense message-major and connection-major, then connection-major groups of kCmGroup - 1,
     kCmGroup and kCmGroup + 1; 64 KiB rings, so a batch carries as many of the topics as fit a ring with
     its wrap padding, and the rings wrap from batch to batch"""
-    guarded(kedges)
     ring = 1 << 16
-    w, keys, topic = edge_world(pcdn, ring_bytes_per_conn=ring, **edge_cfg(pcdn, mode))
+    cfg = layout(pcdn, name)
+    if name.startswith("pool"):
+        cfg["pool_bytes"] = 1 << 30
+    w, keys, topic = edge_world(pcdn, GuardedWorld, ring_bytes_per_conn=ring, delivery=delivery, **cfg)
     tag = 0
     for s in edge_sizes():
         rec = units(s) * K.kUnit
@@ -339,31 +323,33 @@ def test_size_and_recipient_classes_under_guard(pcdn, guarded, mode):
             for d, t in items[i:i + per]:
                 tag += 1
                 w.bcast([t], raw(s, tag))
-            assert kedges.check(w) == sum(d for d, _ in items[i:i + per])
+            assert check(w) == sum(d for d, _ in items[i:i + per])
     cm_len = K.kCmMaxBytes - 4
     dense = EDGE_SLOTS >> K.kCmDenseShift
     for g in (K.kCmGroup - 1, K.kCmGroup, K.kCmGroup + 1):
         for i in range(g):
             tag += 1
             w.bcast([topic[dense + i % 2]], raw(cm_len, tag))
-        assert kedges.check(w) == sum(dense + i % 2 for i in range(g))
+        assert check(w) == sum(dense + i % 2 for i in range(g))
     w.e.close()
+    assert w.guard.verified > 0
 
 
-@pytest.mark.parametrize("out,ctrl,shards", cm_runs.MODES, ids=cm_runs.IDS)
-def test_connection_major_groups_under_guard(pcdn, guarded, out, ctrl, shards):
+@pytest.mark.parametrize("name", CM_MODES, ids=CM_IDS)
+def test_connection_major_groups_under_guard(pcdn, name):
     """test_gpu_cm_runs: partial groups, thin / message-major / direct records inside a group, groups that
     wrap their 16 KiB rings"""
-    guarded(cm_runs)
-    cm_runs.test_groups_that_are_not_one_run(pcdn, out, ctrl, shards)
+    w = workloads.groups_that_are_not_one_run(pcdn, name, world=GuardedWorld)
+    assert w.guard.verified > 0
 
 
-@pytest.mark.parametrize("variant", ["pool", "pool-staged-runs", "pool-host", "pool-shards", "shards-host"])
-def test_random_mixed_batches_under_guard(pcdn, guarded, variant):
+@pytest.mark.parametrize("variant", ["pool", "pool-staged-runs", "pool-host", pytest.param("pool-shards-host", id="pool-shards"),
+                                     "shards-host"])
+def test_random_mixed_batches_under_guard(pcdn, variant):
     """test_gpu_parity's randomized mixed batches (sizes 0 B to 40 KB, fat and thin broadcasts, directs to
     local, remote and unknown keys, state changes between batches)"""
-    guarded(parity)
-    parity.test_random_mixed_batches(pcdn, 0, variant)
+    w = workloads.random_mixed_batches(pcdn, 0, variant, world=GuardedWorld)
+    assert w.guard.verified > 0
 
 
 def test_direct_thresholds_under_guard(pcdn):
@@ -418,6 +404,7 @@ def test_direct_thresholds_under_guard(pcdn):
             send(t[total // 2:])
             assert w.check() > total - 10
     w.e.close()
+    assert w.guard.verified > 0
 
 
 @pytest.mark.parametrize("staged", [False, True])
@@ -466,7 +453,7 @@ def test_e2big_batch_writes_nothing(pcdn):
         assert w.check() == 500
     w.e.handle_broadcast_message([0], orc.broadcast_frame([0], b"too many recipients"))   # the oracle never sees it
     w.check()
-    assert [r.status for r in w.drained] == [E2BIG]
+    assert [r.status for r in w.drained] == [STATUS_E2BIG]
     for rnd in range(3):
         w.bcast([1], orc.broadcast_frame([1], b"more" * 300))
         assert w.check() == 500 and w.e.last_result.n_overflow == 0
@@ -492,9 +479,7 @@ def inflight_world(pcdn, mode):
         cfg.update(flags=pcdn.FLAG_HOST_RINGS)
     elif mode == "shards":
         cfg.update(shard_cfg(pcdn, "shards-host"), max_conns=2048)
-    elif mode == "shared-payload":
-        cfg.update(flags=pcdn.FLAG_SHARED_PAYLOAD)
-    w = GuardedWorld(pcdn, **cfg)
+    w = GuardedWorld(pcdn, delivery="shared" if mode == "shared-payload" else "copy", **cfg)
     n_dense = (3 if mode == "shards" else 1) * w.e.shard_info(0).shard_stride >> K.kCmDenseShift
     for i in range(n_dense + 8):
         w.add_user(b"dense%05d" % i, [0])
@@ -629,7 +614,7 @@ def test_ref_threshold_engine_never_overflows_when_drained(pcdn):
     R = 8192
     T = R - 3                    # round_up(4 + T - 1, 32) == R
     rng = random.Random(17)
-    w = GuardedWorld(pcdn, max_conns=64, ring_bytes_per_conn=R, ref_min_bytes=T)
+    w = GuardedWorld(pcdn, max_conns=64, ring_bytes_per_conn=R, delivery=("ref", T))
     for i in range(48):
         w.add_user(b"r%03d" % i, [i % 3, 3])
     for batch in range(300):
@@ -694,26 +679,25 @@ def test_full_ring_overflows_a_prefix_and_spares_older_batches(pcdn):
     w.e.close()
 
 
-@pytest.mark.parametrize("ctrl,shards", [(c, s) for c in ("fused", "regular") for s in (1, 3)],
-                         ids=["%s-%dshard" % (c, s) for c in ("fused", "regular") for s in (1, 3)])
-def test_overflow_inside_a_connection_major_group_under_guard(pcdn, guarded, ctrl, shards):
+@pytest.mark.parametrize("name", CM_MODES[:4], ids=[i.removeprefix("rings-") for i in CM_IDS[:4]])
+def test_overflow_inside_a_connection_major_group_under_guard(pcdn, name):
     """test_gpu_cm_runs' overflow inside a group, drained under the guard: 20 connection-major records of 34
     units into 512-unit rings; 15 fit, the 16th overflows in the second group of kCmGroup, so the group's
     run must stop there: the 2 units after the 15th record of every dense connection still hold the canary"""
-    guarded(cm_runs)
-    w = cm_runs.world(pcdn, "rings", ctrl, shards)
-    conns = [w.add_user(b"dense%05d" % i, [0]) for i in range(cm_runs.N_DENSE)]
-    frames = [cm_runs.frame([0], t) for t in range(20)]
+    w = cm_world(pcdn, name, GuardedWorld)
+    conns = [w.add_user(b"dense%05d" % i, [0]) for i in range(CM_DENSE)]
+    frames = [cm_frame([0], t) for t in range(20)]
     for f in frames:
         w.e.handle_broadcast_message([0], f)                 # (engine only: the oracle would deliver all 20)
     u = units(len(frames[0]))
-    k = cm_runs.RING // K.kUnit // u
-    assert K.kCmGroup < k < 2 * K.kCmGroup and k * u < cm_runs.RING // K.kUnit
+    k = CM_RING // K.kUnit // u
+    assert K.kCmGroup < k < 2 * K.kCmGroup and k * u < CM_RING // K.kUnit
     got = w.drain()
     rec, = w.drained
     assert sorted(rec.overflow) == sorted(conns)
     for c in conns:
         assert got[c] == frames[:k], c
-        assert uncovered(w, c, k * u, cm_runs.RING // K.kUnit), c
+        assert uncovered(w, c, k * u, CM_RING // K.kUnit), c
     w.guard.verify()
     w.e.close()
+    assert w.guard.verified > 0

@@ -3,9 +3,9 @@
 hash.h they would build none and pass without testing anything, so this test must fail first."""
 import pytest
 
+from gpu_world import PCDN_ENOSPC
 import keyhash as kh
 
-ENOSPC = -5
 SEEDS = [0, 0xF00DFACE12345679]
 MAX_KEYS = 256                      # 128 buckets
 
@@ -34,7 +34,7 @@ def test_nine_keys_on_one_pair_are_refused_on_the_host(pcdn, seed):
     conns = [e.add_user(k) for k in keys[:8]]
     with pytest.raises(pcdn.PcdnError) as ei:
         e.add_user(keys[8])
-    assert ei.value.code == ENOSPC
+    assert ei.value.code == PCDN_ENOSPC
     assert [e.debug_route(k) for k in keys[:8]] == [(1, c) for c in conns]
     assert e.debug_route(keys[8]) == (0, -1)
     assert e.num_users()[0] == 8
@@ -61,7 +61,7 @@ def test_twins_resolve_to_their_own_connections_on_the_host(pcdn, seed):
             e.add_user(k)
         with pytest.raises(pcdn.PcdnError) as ei:
             e.add_user(fill[6])
-        assert ei.value.code == ENOSPC
+        assert ei.value.code == PCDN_ENOSPC
         assert e.debug_route(a) == (1, ca) and e.debug_route(b) == (1, cb)
         e.remove_user(a)
         assert e.debug_route(a) == (0, -1) and e.debug_route(b) == (1, cb)

@@ -5,14 +5,15 @@ import ctypes as C
 
 import pytest
 
-EINVAL = -1
+from gpu_world import PCDN_EINVAL
+
 BASE = dict(device=-1, max_conns=1024, max_keys=1024)
 
 
 def refused(pcdn, **kw):
     with pytest.raises(pcdn.PcdnError) as ei:
         pcdn.Engine(**BASE, **kw)
-    assert ei.value.code == EINVAL
+    assert ei.value.code == PCDN_EINVAL
     return str(ei.value)
 
 

@@ -1,40 +1,12 @@
 """pcdn_send_to_broker / pcdn_send_to_brokers without a GPU: the restatement of Inner::try_send_to_broker /
-try_send_to_brokers (cdn-broker/src/tasks/broker/sender.rs:17-59) on the oracle that the GPU tests compare
-against, the host-only engine's answer and the argument checks that come before it."""
+try_send_to_brokers (cdn-broker/src/tasks/broker/sender.rs:17-59, in gpu_world.py) on the oracle that the GPU tests
+compare against, the host-only engine's answer and the argument checks that come before it."""
 import ctypes as C
 
 import pytest
 
+from gpu_world import PCDN_EINVAL, PCDN_ENODEV, try_send_to_broker, try_send_to_brokers
 from oracle import oracle as orc
-
-ENODEV, EINVAL = -3, -1
-
-
-def relay_key(ident):
-    """a DirectMap key owned by peer broker `ident` (no user key of these tests starts with 0xFF 0x00)"""
-    return b"\xff\x00send-to:" + ident.encode()
-
-
-def try_send_to_broker(o, ident, raw):
-    """Inner::try_send_to_broker (sender.rs:17-45) on oracle `o`; 1 = no such broker (nothing sent).
-    The frame goes through the oracle's own send path: handle_direct_message (tasks/broker/handler.rs:197-237)
-    of a key that `ident` owns ends in try_send_to_broker(ident) → send_message_raw on that broker's connection,
-    so the frame takes its place in the broker's stream in call order with everything routed to it."""
-    if o.broker_conn(ident) < 0:
-        return 1                                       # if let Some(connection) = connection (sender.rs:29)
-    key = relay_key(ident)
-    o.apply_user_sync(ident, [(key, 1, ident)])        # (no local user has the key: nobody is removed)
-    o.handle_direct_message(key, raw)
-    return 0
-
-
-def try_send_to_brokers(o, idents, raw):
-    """Inner::try_send_to_brokers (sender.rs:49-59): try_send_to_broker for every connected broker.  `idents`: the
-    identifiers ever added (the oracle does not list its brokers); 1 = none of them is connected."""
-    live = [i for i in dict.fromkeys(idents) if o.broker_conn(i) >= 0]
-    for i in live:
-        try_send_to_broker(o, i, raw)
-    return 0 if live else 1
 
 
 def framed(raw):
@@ -96,7 +68,7 @@ def test_host_only_engine_refuses_with_enodev(pcdn, sync_frames):
     for call in (lambda: e.send_to_broker("a/a", us), lambda: e.send_to_brokers(us)):
         with pytest.raises(pcdn.PcdnError) as ei:
             call()
-        assert ei.value.code == ENODEV
+        assert ei.value.code == PCDN_ENODEV
         assert "host-only" in e.L.pcdn_last_error().decode()
     e.close()
 
@@ -105,12 +77,12 @@ def test_bad_arguments(pcdn):
     e = pcdn.Engine(device=-1)
     e.add_broker("a/a")
     L = e.L
-    assert L.pcdn_send_to_brokers(e.h, None, 5) == EINVAL
+    assert L.pcdn_send_to_brokers(e.h, None, 5) == PCDN_EINVAL
     assert "null frame" in L.pcdn_last_error().decode()
-    assert L.pcdn_send_to_broker(e.h, b"a/a", None, 1) == EINVAL
+    assert L.pcdn_send_to_broker(e.h, b"a/a", None, 1) == PCDN_EINVAL
     buf = C.create_string_buffer(16)
     # longer than MAX_MESSAGE_SIZE (cdn-proto/src/lib.rs:25): refused before the frame is read
-    assert L.pcdn_send_to_brokers(e.h, C.cast(buf, C.c_char_p), 0x20000000) == EINVAL
+    assert L.pcdn_send_to_brokers(e.h, C.cast(buf, C.c_char_p), 0x20000000) == PCDN_EINVAL
     assert "MAX_MESSAGE_SIZE" in L.pcdn_last_error().decode()
-    assert L.pcdn_send_to_broker(e.h, None, C.cast(buf, C.c_char_p), 0x20000000) == EINVAL
+    assert L.pcdn_send_to_broker(e.h, None, C.cast(buf, C.c_char_p), 0x20000000) == PCDN_EINVAL
     e.close()
